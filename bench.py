@@ -1,19 +1,26 @@
 #!/usr/bin/env python
-"""bench.py — preference-pairs/sec of one full LLaVA-1.5-7B DPO optimisation step on B200.
+"""bench.py — preference-pairs/sec of one full LLaVA-1.5-7B DPO optimisation step on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]            (N=1)
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]            (N=1)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = policy forward on chosen+rejected (CLIP -> projector -> splice -> 32 decoder layers ->
 lm_head -> log-prob gather), DPO loss + gradient, full backward, ZeRO-2 gradient reduction and the
 fused fp32 AdamW, on BASELINE.json configs[1]: 8 synthetic pairs per GPU, 336x336 images,
 48-token prompt + 512-token responses (T = 1135), bf16, random-init weights at true dimensions.
+Full fine-tuning keeps 16 bytes per parameter (bf16 weight + gradient, fp32 master / m / v): 112 GB for the 7 B
+model, sharded over the GPUs by ZeRO-2. Where that does not fit (one 80 GB H100), the headline workload is the LoRA-DPO
+recipe of the same model (BASELINE config e, script/train/llava15_train_lora.sh), which is what one such GPU trains.
 
 `value`  : whole-job pairs/s with the step's inputs already resident in HBM.
 `e2e`    : same metric through the public call DPOStepEngine.train_step() with HOST (pinned) buffers:
            H2D of ids/labels/images/ref-logps and a D2H read of the loss inside the timed region.
-`roofline`: dominant kernel = the tcgen05 GEMM; achieved = sum(2MNK) / sum(CUDA-event durations) of
-           every GEMM launch of one instrumented step, against MEASURED_PEAKS.json.
+`roofline`: dominant kernel = the wgmma GEMM; achieved = sum(2MNK) / sum(CUDA-event durations) of
+           every GEMM launch of one instrumented step, against MEASURED_PEAKS.json if present, else the H100 SXM data
+           sheet (989 TFLOP/s dense bf16, 3.35 TB/s HBM3).
+`--dump-outputs DIR`: after the timed steps, the last timed step's results as DIR/<name>.npy (float32 / float64): the
+           9 metrics train_step returns, and a fixed seeded sample of the trainable parameters (after that step's
+           update) and of their gradients — enough to compare two builds output for output.
 `cpu_baseline` / `--impl reference`: the UNMODIFIED reference staged under oracle/_ref (oracle/stage_ref.py; the
            oracle port only if that staging is absent) on the host cores, on a bounded sample: full-width config-(a)
            steps at 2 and 8 decoder layers after a warm-up, min of 3, extrapolated to 32 layers, raw timings in the
@@ -39,6 +46,9 @@ import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
 PAIRS_PER_GPU = 8
+DATASHEET_BF16_TFLOPS = 989.0      # H100 SXM, dense bf16, 700 W part
+DATASHEET_HBM_GBS = 3350.0
+DUMP_SAMPLE = 1 << 22              # elements per sampled array of --dump-outputs (16 MB as float32)
 PROMPT_LEN, RESP_LEN, IMAGE_POS = 48, 512, 35
 
 
@@ -57,12 +67,12 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 1400.0, 1590.0, "fallback"
+        return d.get("bf16_tflops_sustained", DATASHEET_BF16_TFLOPS), d.get("bf16_tflops", DATASHEET_BF16_TFLOPS), "measured"
+    return DATASHEET_BF16_TFLOPS, DATASHEET_BF16_TFLOPS, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -404,7 +414,7 @@ def run_reference_arm(args, rank):
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": "LLaVA-1.5-7B DPO step, reference CPU path (config (a) shape: 1 pair, 336px, 64-tok "
                                    "responses; full width, 2- and 8-layer steps extrapolated to 32 layers)",
-                       "timed_steps_per_depth": reps, "warmup_steps_per_depth": warm, "same_config_as_b200_arm": False,
+                       "timed_steps_per_depth": reps, "warmup_steps_per_depth": warm, "same_config_as_cuda_arm": False,
                        "note": "BASELINE.json configs[0] is the reference's CPU-runnable case; configs[1] (8 pairs, "
                                "512-tok) would take ~15 min per CPU step"},
             "cpu_baseline": {"value": value, "unit": "pairs/s", "cores": cores, "kind": kind, "sample": sample,
@@ -434,7 +444,27 @@ def eva_flops_per_image(e, batch_tokens=None):
     return e.live_blocks * per_block + 2 * e.n_tokens * e.patch_k * C
 
 
-def run_workload(args, rank, local_rank, world, lora=False, omnilmm=False, steps=None, warmup=None, extras=False):
+def dump_outputs(dump_dir, engine):
+    """The last timed step's results (see the module docstring). The sample indices depend only on the array sizes."""
+    import numpy as np
+    os.makedirs(dump_dir, exist_ok=True)
+    np.save(os.path.join(dump_dir, "metrics.npy"), engine._metrics.double().cpu().numpy())
+    for kind in ("flat", "grad"):
+        parts = [getattr(b, kind).reshape(-1) for b in engine.opt.buckets]
+        n = sum(p.numel() for p in parts)
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randperm(n, generator=g)[:DUMP_SAMPLE].sort().values if n > DUMP_SAMPLE else torch.arange(n)
+        vals, base = [], 0
+        for p in parts:
+            sel = idx[(idx >= base) & (idx < base + p.numel())] - base
+            vals.append(p[sel.to(p.device)].float().cpu())
+            base += p.numel()
+        name = "trainable_params_sample" if kind == "flat" else "trainable_grads_sample"
+        np.save(os.path.join(dump_dir, name + ".npy"), torch.cat(vals).numpy())
+
+
+def run_workload(args, rank, local_rank, world, lora=False, omnilmm=False, steps=None, warmup=None, extras=False,
+                 dump_dir=None):
     """One measured workload -> the JSON line (dict). `extras`: a reduced run used for the `extra` sub-records."""
     from rlaifv_b200 import lib, ops
     from rlaifv_b200.engine import DPOStepEngine
@@ -461,9 +491,9 @@ def run_workload(args, rank, local_rank, world, lora=False, omnilmm=False, steps
     engine = DPOStepEngine(policy, lr=1e-5 if lora else 5e-7, weight_decay=0.01, total_steps=2672, micro_pairs=micro,
                            rank=rank, world=world)
     # HBM plan: with the optimizer state sharded over >= 2 GPUs there is room to stash the normalised inputs
-    # and the SwiGLU product (no recompute in the backward); one GPU holds the unsharded 81 GB state.
+    # and the SwiGLU product (no recompute in the backward)
     policy.stash_extra = world > 1 and not args.no_stash_extra and not (omnilmm and eva is not None)
-    # one GPU, full fine-tuning: room for the SwiGLU product only (peak ~172 of 180 GB); OOM falls back below
+    # one GPU: room for the SwiGLU product at most; OOM falls back below
     policy.stash_act = world == 1 and not lora and not omnilmm and not args.no_stash_extra
     T = PROMPT_LEN + RESP_LEN - 1 + (dims.num_query + 2 if omnilmm else dims.num_patches)
 
@@ -506,22 +536,26 @@ def run_workload(args, rank, local_rank, world, lora=False, omnilmm=False, steps
                 torch.cuda.current_stream().synchronize()
         engine.opt.wait_all()      # the last step's parameter all-gathers belong to the timed region
 
-    try:
-        step0 = engine.train_step(dev_batches[0], optimizer_step=False)   # known-answer check (no update)
-        loss0 = float(step0[0].item())
-    except torch.OutOfMemoryError:
-        # whole-batch activations did not fit next to the optimizer state: fall back to smaller micro-batches
-        policy._stash = None
-        policy._bufs.clear()
-        torch.cuda.empty_cache()
-        if policy.stash_act:
-            policy.stash_act = False            # first give back the optional stash, keep the whole-batch pass
-        else:
-            policy.stash_extra = False
-            micro = max(1, micro // 2)
-            engine.micro_pairs = micro
-        step0 = engine.train_step(dev_batches[0], optimizer_step=False)
-        loss0 = float(step0[0].item())
+    while True:
+        try:
+            step0 = engine.train_step(dev_batches[0], optimizer_step=False)   # known-answer check (no update)
+            loss0 = float(step0[0].item())
+            break
+        except torch.OutOfMemoryError:
+            # the activations did not fit next to the weights / optimizer state: first give back the optional
+            # stashes, then halve the micro-batch
+            policy._stash = None
+            policy._bufs.clear()
+            torch.cuda.empty_cache()
+            if policy.stash_act:
+                policy.stash_act = False
+            elif policy.stash_extra:
+                policy.stash_extra = False
+            elif micro > 1:
+                micro = max(1, micro // 2)
+                engine.micro_pairs = micro
+            else:
+                raise
 
     # ---- device-resident timing (value) ----
     run_steps(dev_batches, warmup, False)
@@ -537,6 +571,8 @@ def run_workload(args, rank, local_rank, world, lora=False, omnilmm=False, steps
     e1.record()
     barrier()
     ms_dev = e0.elapsed_time(e1) / steps
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, engine)
     launches = (lib.launch_count() - launches0) // max(1, steps)
     # ---- end-to-end timing through the public call with host buffers (e2e) ----
     run_steps(host_batches, 1, True)
@@ -597,28 +633,18 @@ def run_workload(args, rank, local_rank, world, lora=False, omnilmm=False, steps
         ops.gemm = orig_gemm
         ops.gemm_dual = orig_dual
         _z.ops.adamw_step = orig_adamw
-    hbm_peak = 6572.2
+    hbm_peak = DATASHEET_HBM_GBS
     pk = os.path.join(REPO, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         with open(pk) as f:
             hbm_peak = json.load(f).get("hbm_gbs", hbm_peak)
-    big = [(s, e, b) for s, e, b in adamw_events if b > 1e9]     # the per-layer buckets (5.7 GB each)
+    big = [(s, e, b) for s, e, b in adamw_events if b > 1e8]     # the large buckets (small ones measure launch latency)
     adamw_gbs = (sum(b for _, _, b in big) / (sum(s.elapsed_time(e) for s, e, _ in big) * 1e-3) / 1e9) if big else None
     gemm_ms = sum(s.elapsed_time(e) for s, e, _ in gemm_events)
     gemm_flops = sum(f for _, _, f in gemm_events)
     peak_sus, peak_burst, peak_kind = measured_peaks()
     achieved = gemm_flops / (gemm_ms * 1e-3) / 1e12
-    # DRAM traffic of the dominant kernel: NOT measured in this run — read from the committed `ncu --set full` capture
-    # (bytes per launch of the forward qkv GEMM; the same capture lists dgrad / wgrad) — profiles/ncu_gemm_traffic.json
-    traffic, traffic_note = None, None
-    tp = os.path.join(REPO, "profiles", "ncu_gemm_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            tj = json.load(f)["gemm"][0]
-        traffic = tj["dram_bytes_per_launch"]
-        traffic_note = "from profiles/ncu_gemm_traffic.json (ncu --set full, not measured in this run): %s: %.3g B DRAM " \
-                       "per launch vs %.3g B algorithmic" % (tj["launch"], tj["dram_bytes_per_launch"],
-                                                             tj["algorithmic_bytes"])
+    traffic, traffic_note = None, "DRAM traffic of the GEMMs: not measured"
 
     total_pairs = B * world
     value = total_pairs / (ms_dev * 1e-3)
@@ -653,31 +679,31 @@ def run_workload(args, rank, local_rank, world, lora=False, omnilmm=False, steps
                    "layers": args.layers, "pairs_per_gpu": B, "micro_pairs": micro, "parallelism": "dp%d" % world,
                    "stash_extra": bool(policy.stash_extra), "stash_act": bool(policy.stash_act),
                    "compact_head": bool(policy.compact_head),
-                   "l2": "per-step working set (>100 GB of weights/activations) is far larger than the 126 MB L2",
+                   "l2": "per-step working set (tens of GB of weights/activations) is far larger than the 50 MB L2",
                    "step0_loss": loss0, "step0_loss_expected": math.log(2.0)},
         "e2e": {"value": e2e_value, "unit": "pairs/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 36,
                 "ms_per_step": ms_e2e},
         "hbm_peak_gb": torch.cuda.max_memory_allocated() / 2 ** 30,
         "gpu_launches": int(launches), "host_enqueue_ms_per_step": host_enqueue_ms,
-        "host_enqueue_note": "wall time of the enqueue loop INCLUDING blocking on the full launch queue; the real host "
-                             "work is ~12 us per launch (profiles/r02_host_overhead.log: 13 ms per step)",
+        "host_enqueue_note": "wall time of the enqueue loop INCLUDING blocking on the full launch queue",
         "clocks": clocks,
         "model_flops_per_pair": f_pair,
         "step_tflops_per_gpu": value / world * f_pair / 1e12,
-        "step_frac_of_peak": {"measured_sustained_%g" % peak_sus: value / world * f_pair / 1e12 / peak_sus,
-                              "measured_burst_%g" % peak_burst: value / world * f_pair / 1e12 / peak_burst,
-                              "datasheet_2250": value / world * f_pair / 1e12 / 2250.0},
-        "roofline": {"bound": "tensor", "kernel": "gemm2_bf16_kernel / gemm_bf16_kernel (tcgen05, all GEMM launches of a step)", "achieved": achieved,
+        "step_frac_of_peak": dict(({"measured_sustained_%g" % peak_sus: value / world * f_pair / 1e12 / peak_sus,
+                                    "measured_burst_%g" % peak_burst: value / world * f_pair / 1e12 / peak_burst}
+                                   if peak_kind == "measured" else {}),
+                                  **{"datasheet_%g" % DATASHEET_BF16_TFLOPS:
+                                     value / world * f_pair / 1e12 / DATASHEET_BF16_TFLOPS}),
+        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel (wgmma, all GEMM launches of a step)", "achieved": achieved,
                      "peak": peak_sus, "unit": "TFLOP/s", "frac": achieved / peak_sus, "traffic": traffic, "traffic_note": traffic_note,
-                     "peak_source": "%s bf16_tflops_sustained (kernel timed inside a long step); burst %g"
-                                    % (peak_kind, peak_burst),
+                     "peak_source": ("measured bf16_tflops_sustained (MEASURED_PEAKS.json); burst %g" % peak_burst
+                                     if peak_kind == "measured" else peak_kind),
                      "frac_of_burst": achieved / peak_burst,
-                     "frac_note": "the sustained figure is a cuBLAS 8192^3 matmul run back to back under the same power "
-                                  "cap — a library measurement, not a hardware bound, so frac can exceed 1 when this "
-                                  "kernel moves fewer bytes per FLOP; frac_of_burst relates it to the same matmul timed alone",
+                     "frac_note": "achieved over the peak named in peak_source (a data-sheet rate is not a measured "
+                                  "one: a power-limited card runs below it)",
                      "gemm_launches": len(gemm_events), "gemm_ms_per_step": gemm_ms,
                      "gemm_share_of_step": gemm_ms / ms_dev},
-        "roofline_hbm": {"bound": "hbm", "kernel": "adamw_kernel (fused AdamW on a 202M-parameter layer bucket)",
+        "roofline_hbm": {"bound": "hbm", "kernel": "adamw_kernel (fused AdamW on the large parameter buckets)",
                          "achieved": adamw_gbs, "peak": hbm_peak, "unit": "GB/s",
                          "frac": (adamw_gbs / hbm_peak) if adamw_gbs else None,
                          "note": "28 algorithmic bytes per parameter; timed on the optimizer side stream while the "
@@ -716,8 +742,12 @@ def main():
                     help="BASELINE config (d) as the (only) workload: EVA tower + resampler + Mistral-7B GQA decoder "
                          "(11.6 B trainable parameters: needs >= 2 GPUs for the ZeRO-2 sharded fp32 optimizer state)")
     ap.add_argument("--omnilmm-no-tower", action="store_true",
-                    help="with --omnilmm: feed the tower's output tokens (the round-1 boundary; fits one GPU)")
+                    help="with --omnilmm: feed the tower's output tokens (the decoder side alone)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results as DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
+    if args.steps < 1:
+        raise SystemExit("--steps must be >= 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -732,19 +762,26 @@ def main():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
 
-    line = run_workload(args, rank, local_rank, world, lora=args.lora, omnilmm=args.omnilmm)
     headline = not (args.lora or args.omnilmm)
+    # full fine-tuning state of the 7 B model (16 B per parameter), ZeRO-2-sharded, plus ~20 GB of activations
+    full_ft_fits = 16 * 7.06e9 / world + 20 * 2 ** 30 <= torch.cuda.get_device_properties(local_rank).total_memory
+    lora = args.lora or (headline and not full_ft_fits)
+    line = run_workload(args, rank, local_rank, world, lora=lora, omnilmm=args.omnilmm, dump_dir=args.dump_outputs)
+    if headline and not full_ft_fits:
+        line["config"]["full_finetune"] = ("not run: 16 B x 7.06 B parameters / %d GPU(s) of fp32 optimizer state, bf16 "
+                                           "weights and gradients do not fit %.0f GB; the LoRA-DPO step is the headline"
+                                           % (world, torch.cuda.get_device_properties(local_rank).total_memory / 2 ** 30))
     if headline and not args.no_extras:
-        # BASELINE configs (e) and (d) as driver-visible sub-records of the same run (short: 3 timed steps each).
+        # BASELINE configs (e) and (d) as sub-records of the same run (short: 3 timed steps each).
         # Every rank runs them (collectives inside); a failure is recorded, never raised.
         extra = {}
-        plan = [("lora_dpo_config_e", dict(lora=True, omnilmm=False))]
+        plan = [("lora_dpo_config_e", dict(lora=True, omnilmm=False))] if not lora else []
         if world >= 2:
             plan.append(("omnilmm_12b_config_d", dict(lora=False, omnilmm=True)))
         else:
             extra["omnilmm_12b_config_d"] = {
                 "unavailable": "11.6 B trainable parameters x 16 B (bf16 param + grad, fp32 master/m/v) = 186 GB do not "
-                               "fit one 180 GB GPU; measured at N >= 2 (ZeRO-2 shards the 139 GB optimizer state)"}
+                               "fit one GPU; needs N >= 4 80 GB GPUs (ZeRO-2 shards the 139 GB optimizer state)"}
         for name, kw in plan:
             try:
                 sub = run_workload(args, rank, local_rank, world, steps=3, warmup=2, extras=True, **kw)

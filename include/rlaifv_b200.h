@@ -1,4 +1,4 @@
-/* rlaifv_b200.h — C ABI of librlaifv_b200.so: the B200 (sm_100a) kernels of the LLaVA-1.5 DPO
+/* rlaifv_b200.h — C ABI of librlaifv_b200.so: the H100 (sm_90a) kernels of the LLaVA-1.5 DPO
  * training step that replaces the reference's HF/torch hot path.
  *
  * Conventions
@@ -22,11 +22,12 @@ extern "C" {
 
 const char* rlaifv_last_error(void);
 
-/* ---- dense contractions (tcgen05 / TMA) -------------------------------------------------------
+/* ---- dense contractions (wgmma / TMA) ----------------------------------------------------------
  * C[M,N] (+)= op(A) * op(B)^T (+ bias[N]) -> act -> (+ residual[M,N]).
  *   a_mn_major = 0: A is [M][K] (K contiguous)      1: A is stored [K][M]
  *   b_mn_major = 0: B is [N][K] (K contiguous)      1: B is stored [K][N]
- *   act: 0 none, 1 GELU(erf), 2 quick_gelu.  accumulate: C += result.  tile_n: 0 auto, 128, 256.
+ *   act: 0 none, 1 GELU(erf), 2 quick_gelu.  accumulate: C += result.  tile_n: 0 auto, 128, 256, or 512 = a
+ *   256x256 tile per 2-CTA cluster (each CTA 128 rows; the B operand is TMA-multicast to both).
  * Replaces every nn.Linear forward / dgrad / wgrad of HF LlamaDecoderLayer (HF:llama/modeling_llama.py
  * :182-184,:262-264,:289), lm_head (llava/model/language_model/llava_llama.py:91-102), CLIP layers
  * (HF:clip/modeling_clip.py:300-351), the patch-embedding conv as im2col GEMM (:148-154) and the
@@ -62,14 +63,11 @@ int rlaifv_gemm_bf16_swiglu_bwd(const void* A, long long lda, const void* B, lon
                                 const void* A2, long long lda2, const void* B2, long long ldb2, int K2, const void* gu,
                                 long long ld_gu, void* dgu, long long ld_dgu, int M, int F, int K, void* stream);
 
-/* tile_n = 512 selects the 2-CTA kernel (cta_group::2, 256x256 tile per CTA pair). rlaifv_gemm_set_2cta(1)
- * lets tile_n = 0 (auto) pick it for large problems. */
-int rlaifv_gemm_set_2cta(int enable);
-/* raster group size (row-blocks per group, default 16) and profiling switches (debug: bit0 skip stores,
- * bit1 skip TMEM loads too — results are then garbage; for roofline experiments only). */
+/* raster group size (row-blocks per group, default 16) and a profiling switch (debug: bit0 skip the stores of C —
+ * results are then garbage; for roofline experiments only). */
 int rlaifv_gemm_set_tuning(int group_m, int debug);
-/* L2 policy of the CTA-pair kernel's TMA traffic: bits 0-1 A loads, 2-3 B loads, 4-5 C stores (0 normal, 1 evict
- * first, 2 evict last); bit 6: raster walks n-fastest inside groups of group_m column blocks instead of m-fastest
+/* L2 policy of the GEMM's TMA operand loads: bits 0-1 A loads, 2-3 B loads (0 normal, 1 evict first, 2 evict last;
+ * bits 4-5 are accepted and ignored); bit 6: raster walks n-fastest inside groups of group_m column blocks instead of m-fastest
  * inside groups of row blocks. l2 < 0 (default): raster, group size and hints are chosen per launch from the shape
  * (long-K launches keep the smaller operand's panels resident in the L2); l2 >= 0 forces the given bits together
  * with rlaifv_gemm_set_tuning's group size. Process-wide; results are unaffected. */
@@ -77,11 +75,6 @@ int rlaifv_gemm_set_l2(int l2);
 /* EXPERIMENTAL (default off): run GEMMs with K >= min_k and no bias / activation / residual as n K-slice passes
  * (passes 2.. with C +=) so each pass's operand slabs fit the L2. n <= 1 switches it off. */
 int rlaifv_gemm_set_split_k(int n, int min_k);
-
-/* Forward-kernel selection (tuning / A-B only): 1 (default) = two query tiles per CTA ping-ponging between the
- * softmax warpgroups and the tensor pipe, P kept in TMEM as the A operand of the PV MMA; 0 = the round-1 single-tile
- * kernel (P through shared memory). Results agree to fp32 rounding of the online softmax. */
-int rlaifv_attention_set_variant(int fwd_variant);
 
 /* Split attention backward (default for self-attention; replaces HF autograd through the eager attention of
  * llama/modeling_llama.py:199-222): attention_bwd_dkv_kernel (dK, dV per 128-row K/V tile) + attention_bwd_dq_kernel
@@ -96,7 +89,7 @@ int rlaifv_attention_bwd_split(const void* q, long long ld_q, const void* k, con
                                void* stream);
 
 
-/* ---- attention (tcgen05, S/O accumulators in TMEM) ---------------------------------------------
+/* ---- attention (wgmma, S/O accumulators in registers) -----------------------------------------
  * q/k/v/out: [nseq*S][ld] bf16, head h at columns [h*head_dim, (h+1)*head_dim); lse fp32
  * [nseq][n_heads][S]. head_dim 128 (Llama, causal) or 64 (CLIP, non-causal).
  * Replaces HF:llama/modeling_llama.py:199-222 (eager causal attention; attention_mask=None as set at
@@ -113,7 +106,7 @@ int rlaifv_attention_bwd(const void* q, const void* k, const void* v, long long 
 
 /* Grouped-query variants (Mistral-7B decoder of OmniLMM-12B, omnilmm/model/omnilmm.py:259-265 -> HF
  * MistralForCausalLM: 32 query / 8 key-value heads): k/v (and dk/dv) hold n_kv_heads heads; query head h uses
- * kv head h / (n_heads / n_kv_heads); the backward sums the group's dK/dV contributions in TMEM. */
+ * kv head h / (n_heads / n_kv_heads); the backward sums the group's dK/dV contributions in registers. */
 int rlaifv_attention_fwd_gqa(const void* q, const void* k, const void* v, long long ld_qkv, void* out,
                              long long ld_out, float* lse, int nseq, int S, int n_heads, int n_kv_heads,
                              int head_dim, int causal, float scale, void* stream);

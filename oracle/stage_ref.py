@@ -44,7 +44,7 @@ def stage(force=False, verbose=False):
         if os.path.isdir(TARGET):
             shutil.rmtree(TARGET)
         cmd = [sys.executable, "-m", "pip", "install", "--no-index", "--no-build-isolation", "--no-deps", "--quiet",
-               "--find-links", "/opt/wheelhouse", "--target", TARGET, src]
+               "--target", TARGET, src]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             if verbose:

@@ -1,8 +1,8 @@
-"""Build the C-ABI CUDA library in-tree for sm_100a (nvcc cross-compiles without a GPU).
+"""Build the C-ABI CUDA library in-tree for sm_90a (H100; nvcc cross-compiles without a GPU).
 
     python rlaif-v_b200/build.py [--force]
 
-Output: rlaif-v_b200/librlaifv_b200.so (git-ignored; travels to the GPU box with the snapshot).
+Output: rlaif-v_b200/librlaifv_b200.so (git-ignored build product).
 """
 import hashlib
 import os
@@ -16,7 +16,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "librlaifv_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
 

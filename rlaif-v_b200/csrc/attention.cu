@@ -1,19 +1,17 @@
-// Fused attention for sm_100a on tcgen05: S = Q K^T and O += P V run on the 5th-gen tensor cores with the S / O
-// accumulators in TMEM; softmax is done one-thread-per-query-row straight out of TMEM (no shuffles).
+// Fused attention for sm_90a on wgmma: S = Q K^T and O += P V run on the warpgroup tensor cores with the S / O
+// accumulators in registers; P never leaves the registers (it is the A operand of the PV wgmma). K / V (or Q / dO)
+// stream through a TMA-fed two-stage shared-memory ring.
 //
-//   forward  (attention_fwd2_kernel, default): two 128-row query tiles per CTA ping-pong against the tensor pipe; P is
-//             packed back into its own S columns and consumed as the TMEM A operand of the PV MMA. Causal d=128
-//             (Llama; HF llama/modeling_llama.py:199-222, attention_mask=None => pure causal, pads attended —
-//             muffin/train/trainers.py:199), non-causal d=64 (CLIP; HF clip/modeling_clip.py:261-279) and d=128
-//             (EVA tower, heads padded 112 -> 128). Softmax in fp32, P rounded to bf16 before PV.
-//             attention_fwd_kernel is the round-1 single-tile kernel (P through shared memory), still selectable.
-//   backward (attention_bwd_dkv_kernel + attention_bwd_dq_kernel, default): dK/dV per 128-row K/V tile, dQ per
-//             128-row Q tile, both streaming 64-row chunks of the other side; S^T / dP^T (S / dP) are recomputed per
-//             chunk, P^T / dS^T / dS go back into the TMEM columns they came from as A operands; no atomics, dQ is
-//             written once as bf16. attention_bwd_kernel is the fused round-1 kernel (five MMAs per tile pair, dQ
-//             reduced with fp32 red.global.add); it serves the resampler's shared-query cross-attention.
-//   Epilogues stage each warp's 32 rows in shared memory and write whole rows (store_tile_rows).
+//   forward  (attention_fwd_kernel): one CTA per (128-row query tile, head, sequence). Causal d=128 (Llama; HF
+//             llama/modeling_llama.py:199-222, attention_mask=None => pure causal, pads attended —
+//             muffin/train/trainers.py:199), non-causal d=64 (CLIP; HF clip/modeling_clip.py:261-279) and d=128 (EVA
+//             tower, heads padded 112 -> 128; resampler cross-attention). Softmax in fp32, P rounded to bf16 before PV.
+//   backward (attention_bwd_dkv_kernel + attention_bwd_dq_kernel): dK/dV per 128-row K/V tile streaming 64-row chunks
+//             of Q / dO, dQ per 128-row Q tile streaming 64-row chunks of K / V; S / dP are recomputed in each. dQ is
+//             written once as bf16, or reduced into an fp32 buffer (the resampler's shared queries sum over images).
 //
+// Warp roles (288 threads): warpgroups 0, 1 = math, 64 rows each (thread = two rows of the wgmma accumulator layout,
+// see common.cuh); warp 8 = TMA producer (one thread issues).
 // Layouts: q/k/v/o are [nseq*S rows][ld] bf16 with head h at columns [h*D, h*D+D); q, k, v may be
 // column blocks of one fused qkv buffer. LSE is fp32 [nseq][n_heads][S] (natural log).
 #include "common.cuh"
@@ -23,6 +21,8 @@ namespace b200 {
 
 constexpr int ATT_BQ = 128;
 constexpr int ATT_BKV = 128;
+constexpr int ATT_THREADS = 288;   // two math warpgroups + one producer warp
+constexpr int ATT_STAGES = 2;
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
 
@@ -32,43 +32,54 @@ __device__ __forceinline__ float fast_exp2(float x) {   // MUFU.EX2, flush-to-ze
   return y;
 }
 
-// One warp writes its 32 rows x (NCH*32) bf16 columns — held in TMEM as fp32, one row per lane — to global memory with
-// coalesced stores. The row-per-lane form (each lane writes 16-byte pieces of its own row) makes every store
-// instruction touch 32 different rows; with one CTA per SM nothing overlaps the epilogue and ncu showed the compute
-// warps of the backward kernels spending 18-26 % of their time there. Each row is staged as NCH*64 bytes in a per-warp
-// shared buffer (16-byte chunks XOR-swizzled by the row so that neither the row-per-lane writes nor the row-major
-// reads conflict), then every instruction writes whole rows: 2 rows x 256 bytes (D = 128) or 4 x 128 bytes.
-// `mul` scales the row (1/l in the forward), `rows_valid` clips the rows beyond the sequence end.
-template <int NCH>
-__device__ __forceinline__ void store_tile_rows(uint32_t taddr, float mul, uint8_t* stage, int lane, bf16* g_row0,
-                                                long long ld, int rows_valid) {
-  constexpr int ROW_B = NCH * 64;            // bytes per staged row
-  constexpr int CPR = ROW_B / 16;            // 16-byte chunks per row
-  constexpr int RPI = 32 / CPR;              // rows per store instruction
-#pragma unroll 1
-  for (int ch = 0; ch < NCH; ++ch) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(taddr + ch * 32, v);
-    tmem_wait_ld();
+// the two rows of the 64-row block a thread holds, and its first column in every 8-column group
+struct FragPos {
+  int r0;   // row of d[4i], d[4i+1]; row r0 + 8 holds d[4i+2], d[4i+3]
+  int c0;   // column of d[4i] is 8i + c0
+};
+__device__ __forceinline__ FragPos frag_pos() {
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  return FragPos{w * 16 + (lane >> 2), (lane & 3) * 2};
+}
+
+// wgmma accumulator of a 64 x (16*KS) tile -> bf16 A fragments of KS k16 steps
+template <int KS>
+__device__ __forceinline__ void acc_to_afrag(const float* d, uint32_t (&a)[KS][4]) {
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      uint4 u;
-      u.x = pack_bf16(__uint_as_float(v[g * 8 + 0]) * mul, __uint_as_float(v[g * 8 + 1]) * mul);
-      u.y = pack_bf16(__uint_as_float(v[g * 8 + 2]) * mul, __uint_as_float(v[g * 8 + 3]) * mul);
-      u.z = pack_bf16(__uint_as_float(v[g * 8 + 4]) * mul, __uint_as_float(v[g * 8 + 5]) * mul);
-      u.w = pack_bf16(__uint_as_float(v[g * 8 + 6]) * mul, __uint_as_float(v[g * 8 + 7]) * mul);
-      const int c = ch * 4 + g;
-      *reinterpret_cast<uint4*>(stage + lane * ROW_B + ((c ^ (lane & (CPR - 1))) << 4)) = u;
-    }
+  for (int k = 0; k < KS; ++k) {
+    a[k][0] = pack_bf16(d[8 * k + 0], d[8 * k + 1]);
+    a[k][1] = pack_bf16(d[8 * k + 2], d[8 * k + 3]);
+    a[k][2] = pack_bf16(d[8 * k + 4], d[8 * k + 5]);
+    a[k][3] = pack_bf16(d[8 * k + 6], d[8 * k + 7]);
   }
-  __syncwarp();
+}
+
+// S[64 x 64*NB] = A[64 rows of a K-major tile] * B[64*NB rows of a K-major tile]^T over D (both stored as D/64 atoms)
+template <int D>
+__device__ __forceinline__ void mma_qk_64(float (&s)[32], uint32_t a_addr, uint32_t a_atom, uint32_t b_addr,
+                                          uint32_t b_atom) {
 #pragma unroll
-  for (int it = 0; it < 32 / RPI; ++it) {
-    const int r = it * RPI + lane / CPR, c = lane % CPR;
-    const uint4 u = *reinterpret_cast<const uint4*>(stage + r * ROW_B + ((c ^ (r & (CPR - 1))) << 4));
-    if (r < rows_valid) *reinterpret_cast<uint4*>(g_row0 + (long long)r * ld + c * 8) = u;
+  for (int k16 = 0; k16 < D / 16; ++k16)
+    wgmma_m64n64_ss<0, 0>(s, desc_kmajor(a_addr + (k16 >> 2) * a_atom, k16 & 3),
+                          desc_kmajor(b_addr + (k16 >> 2) * b_atom, k16 & 3), k16 > 0);
+}
+template <int D>
+__device__ __forceinline__ void mma_qk_128(float (&s)[64], uint32_t a_addr, uint32_t a_atom, uint32_t b_addr,
+                                           uint32_t b_atom) {
+#pragma unroll
+  for (int k16 = 0; k16 < D / 16; ++k16)
+    wgmma_m64n128_ss<0, 0>(s, desc_kmajor(a_addr + (k16 >> 2) * a_atom, k16 & 3),
+                           desc_kmajor(b_addr + (k16 >> 2) * b_atom, k16 & 3), k16 > 0);
+}
+// O[64 x D] += P[64 x 16*KS] (registers) * V[16*KS rows][D] (MN-major B: D/64 atoms of [rows][64], atom stride given)
+template <int D, int KS>
+__device__ __forceinline__ void mma_pv(float (&o)[D / 2], const uint32_t (&p)[KS][4], uint32_t v_addr,
+                                       uint32_t v_atom) {
+#pragma unroll
+  for (int k = 0; k < KS; ++k) {
+    if constexpr (D == 128) wgmma_m64n128_rs<1>(o, p[k], desc_mnmajor(v_addr, k, v_atom), 1);
+    else wgmma_m64n64_rs<1>(o, p[k], desc_mnmajor(v_addr, k, v_atom), 1);
   }
-  __syncwarp();
 }
 
 // ================================================================================================
@@ -76,20 +87,18 @@ __device__ __forceinline__ void store_tile_rows(uint32_t taddr, float mul, uint8
 // ================================================================================================
 template <int D>
 struct AttFwdCfg {
+  static constexpr uint32_t Q_ATOM = ATT_BQ * 128;           // [128 rows][64 cols]
+  static constexpr uint32_t KV_ATOM = ATT_BKV * 128;
   static constexpr uint32_t Q_BYTES = ATT_BQ * D * 2;
-  static constexpr uint32_t KV_BYTES = ATT_BKV * D * 2;   // one of K or V
-  static constexpr uint32_t P_BYTES = ATT_BQ * ATT_BKV * 2;
-  static constexpr uint32_t OFF_Q = 0;
-  static constexpr uint32_t OFF_K = Q_BYTES;                  // 2 stages
-  static constexpr uint32_t OFF_V = OFF_K + 2 * KV_BYTES;     // 2 stages
-  static constexpr uint32_t OFF_P = OFF_V + 2 * KV_BYTES;
-  static constexpr uint32_t OFF_BAR = OFF_P + P_BYTES;
+  static constexpr uint32_t KV_BYTES = ATT_BKV * D * 2;      // one of K or V
+  static constexpr uint32_t OFF_K = Q_BYTES;                 // [STAGES]
+  static constexpr uint32_t OFF_V = OFF_K + ATT_STAGES * KV_BYTES;
+  static constexpr uint32_t OFF_BAR = OFF_V + ATT_STAGES * KV_BYTES;
   static constexpr uint32_t SMEM_BYTES = OFF_BAR + 128 + 1024;
-  static constexpr uint32_t TMEM_COLS = 256;  // S: [0,128), O: [128,128+D)
 };
 
 template <int D, bool CAUSAL>
-__global__ void __launch_bounds__(160, 1)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, bf16* __restrict__ out, long long ld_out,
                      float* __restrict__ lse_out, int Sq, int Skv, int n_heads, int kv_group, int q_shared,
@@ -103,503 +112,143 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* q_full = bars + 0;
-  uint64_t* kv_full = bars + 1;   // [2]
-  uint64_t* kv_empty = bars + 3;  // [2]
-  uint64_t* s_full = bars + 5;
-  uint64_t* p_full = bars + 6;
-  uint64_t* o_done = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;                 // [STAGES]
+  uint64_t* kv_empty = bars + 1 + ATT_STAGES;   // [STAGES]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const int num_q_tiles = (Sq + ATT_BQ - 1) / ATT_BQ;
   const int q_tile = num_q_tiles - 1 - blockIdx.x;  // heavy (late) tiles first
   const int head = blockIdx.y, seq = blockIdx.z;
   const int q_seq = q_shared ? 0 : seq;
   const int kv_head = head / kv_group;
   const int q0 = q_tile * ATT_BQ;
-  const int n_kv = CAUSAL ? (q_tile + 1) : (Skv + ATT_BKV - 1) / ATT_BKV;
+  const int n_kv_all = (Skv + ATT_BKV - 1) / ATT_BKV;
+  const int n_kv = CAUSAL ? min(n_kv_all, (q0 + ATT_BQ + ATT_BKV - 1) / ATT_BKV) : n_kv_all;
 
-  if (warp == 4) {
-    if (lane == 0) {
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int i = 0; i < ATT_STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    // ------------------------------ TMA producer ------------------------------
+    if (threadIdx.x == 256) {
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmK);
       tma_prefetch_desc(&tmV);
-      mbar_init(q_full, 1);
-      for (int i = 0; i < 2; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-      mbar_init(s_full, 1);
-      mbar_init(p_full, 128);
-      mbar_init(o_done, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_O = tmem_base + 128;
-
-  if (warp == 4) {
-    // ------------------------------ control: TMA + MMA issue ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, ATT_BKV, false, false);
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, D, false, true);
-      const uint32_t q_addr = smem_u32(smem + Cfg::OFF_Q);
-      const uint32_t p_addr = smem_u32(smem + Cfg::OFF_P);
-      auto load_kv = [&](int j) {
-        const int s = j & 1;
-        mbar_arrive_expect_tx(&kv_full[s], 2 * Cfg::KV_BYTES);
-#pragma unroll
-        for (int a = 0; a < D / 64; ++a) {
-          tma_load_3d(smem + Cfg::OFF_K + s * Cfg::KV_BYTES + a * (ATT_BKV * 128), &tmK, &kv_full[s],
-                      kv_head * D + a * 64, j * ATT_BKV, seq);
-          tma_load_3d(smem + Cfg::OFF_V + s * Cfg::KV_BYTES + a * (ATT_BKV * 128), &tmV, &kv_full[s],
-                      kv_head * D + a * 64, j * ATT_BKV, seq);
-        }
-      };
-      auto issue_s = [&](int j) {
-        const int s = j & 1;
-        mbar_wait(&kv_full[s], (j >> 1) & 1);
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(smem + Cfg::OFF_K + s * Cfg::KV_BYTES);
-#pragma unroll
-        for (int k16 = 0; k16 < D / 16; ++k16) {
-          const uint64_t ad = desc_kmajor(q_addr + (k16 >> 2) * (ATT_BQ * 128), k16 & 3);
-          const uint64_t bd = desc_kmajor(k_addr + (k16 >> 2) * (ATT_BKV * 128), k16 & 3);
-          umma_ss(tmem_S, ad, bd, idesc_s, k16 > 0 ? 1u : 0u);
-        }
-        umma_commit(s_full);
-      };
       mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
 #pragma unroll
       for (int a = 0; a < D / 64; ++a)
-        tma_load_3d(smem + Cfg::OFF_Q + a * (ATT_BQ * 128), &tmQ, q_full, head * D + a * 64, q0, q_seq);
-      load_kv(0);
-      if (n_kv > 1) load_kv(1);
-      mbar_wait(q_full, 0);
-      issue_s(0);
+        tma_load_3d(smem + a * Cfg::Q_ATOM, &tmQ, q_full, head * D + a * 64, q0, q_seq);
       for (int j = 0; j < n_kv; ++j) {
-        const int s = j & 1;
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        const uint32_t v_addr = smem_u32(smem + Cfg::OFF_V + s * Cfg::KV_BYTES);
+        const int s = j % ATT_STAGES;
+        if (j >= ATT_STAGES) mbar_wait(&kv_empty[s], ((j / ATT_STAGES) - 1) & 1);
+        mbar_arrive_expect_tx(&kv_full[s], 2 * Cfg::KV_BYTES);
 #pragma unroll
-        for (int k16 = 0; k16 < ATT_BKV / 16; ++k16) {
-          const uint64_t ad = desc_kmajor(p_addr + (k16 >> 2) * (ATT_BQ * 128), k16 & 3);
-          const uint64_t bd = desc_mnmajor(v_addr, k16, ATT_BKV);
-          umma_ss(tmem_O, ad, bd, idesc_o, (j > 0 || k16 > 0) ? 1u : 0u);
-        }
-        umma_commit(&kv_empty[s]);
-        umma_commit(o_done);
-        if (j + 1 < n_kv) {
-          issue_s(j + 1);
-          if (j + 2 < n_kv) {
-            mbar_wait(&kv_empty[s], (j >> 1) & 1);
-            load_kv(j + 2);
-          }
+        for (int a = 0; a < D / 64; ++a) {
+          tma_load_3d(smem + Cfg::OFF_K + s * Cfg::KV_BYTES + a * Cfg::KV_ATOM, &tmK, &kv_full[s],
+                      kv_head * D + a * 64, j * ATT_BKV, seq);
+          tma_load_3d(smem + Cfg::OFF_V + s * Cfg::KV_BYTES + a * Cfg::KV_ATOM, &tmV, &kv_full[s],
+                      kv_head * D + a * 64, j * ATT_BKV, seq);
         }
       }
     }
   } else {
-    // ------------------------------ softmax / epilogue: one thread per query row ------------------------------
-    const int r = warp * 32 + lane;          // row in tile == TMEM lane
-    const int q_idx = q0 + r;
-    const uint32_t lane_off = (uint32_t)(warp * 32) << 16;
+    // ------------------------------ softmax / PV: rows [64*wg, 64*wg + 64) of the query tile ------------------------
+    const FragPos fp = frag_pos();
+    const int qr[2] = {q0 + wg * 64 + fp.r0, q0 + wg * 64 + fp.r0 + 8};
     const float c = scale * LOG2E;
-    float m_used = -INFINITY, l = 0.f;
-    uint8_t* p_row = smem + Cfg::OFF_P + r * 128;
+    float o[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    const uint32_t q_addr = smem_u32(smem) + wg * 64 * 128;
+    mbar_wait(q_full, 0);
     for (int j = 0; j < n_kv; ++j) {
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
+      const int s = j % ATT_STAGES;
+      mbar_wait(&kv_full[s], (j / ATT_STAGES) & 1);
+      const uint32_t k_addr = smem_u32(smem + Cfg::OFF_K + s * Cfg::KV_BYTES);
+      const uint32_t v_addr = smem_u32(smem + Cfg::OFF_V + s * Cfg::KV_BYTES);
+      float sv[64];
+      wgmma_fence();
+      mma_qk_128<D>(sv, q_addr, Cfg::Q_ATOM, k_addr, Cfg::KV_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(sv);
       const int kv0 = j * ATT_BKV;
-      const bool need_mask = (kv0 + ATT_BKV > Skv) || (CAUSAL && j == q_tile);
-      // single pass over S: the whole 128-column row is pulled into registers with two async
-      // TMEM loads (one wait), then max / exp2 / pack run from registers.
-      uint32_t v[128];
-      tmem_ld_32x32b_x64(tmem_S + lane_off, v);
-      tmem_ld_32x32b_x64(tmem_S + lane_off + 64, v + 64);
-      tmem_wait_ld();
-      if (need_mask) {
+      if (kv0 + ATT_BKV > Skv || (CAUSAL && kv0 + ATT_BKV - 1 > q0 + wg * 64)) {
 #pragma unroll
-        for (int i = 0; i < 128; ++i) {
-          const int kv = kv0 + i;
-          if ((kv >= Skv) || (CAUSAL && kv > q_idx)) v[i] = 0xff800000u;   // -inf
-        }
-      }
-      float mx = -INFINITY;
+        for (int i = 0; i < 16; ++i)
 #pragma unroll
-      for (int i = 0; i < 128; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-      float m_new = fmaxf(m_used, mx * c);
-      if (m_new == -INFINITY) m_new = 0.f;
-      if (j == 0) {
-        m_used = m_new;
-      } else {
-        const bool need = (m_new - m_used) > 8.0f;
-        mbar_wait(o_done, (j - 1) & 1);  // PV_{j-1} finished: O readable, P smem reusable
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {
-          const float alpha = need ? fast_exp2(m_used - m_new) : 1.f;
-          if (need) { m_used = m_new; l *= alpha; }
-#pragma unroll 1
-          for (int ch = 0; ch < D / 32; ++ch) {
-            uint32_t o[32];
-            tmem_ld_32x32b_x32(tmem_O + lane_off + ch * 32, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32b_x32(tmem_O + lane_off + ch * 32, o);
+          for (int e = 0; e < 4; ++e) {
+            const int kv = kv0 + 8 * i + fp.c0 + (e & 1);
+            if (kv >= Skv || (CAUSAL && kv > qr[e >> 1])) sv[4 * i + e] = -INFINITY;
           }
-          tmem_wait_st();
-        }
       }
-      // P = exp2(s*c - m) -> bf16 -> swizzled smem (A operand of the PV MMA); row sum in fp32
-      float rs = 0.f;
+      // online softmax, two rows per thread; a row's 128 columns are spread over the 4 lanes of a quad
+      float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int g = 0; g < 16; ++g) {
-        float p[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          p[i] = fast_exp2(__uint_as_float(v[g * 8 + i]) * c - m_used);   // exp2(-inf) = 0 for masked
-          rs += p[i];
-        }
-        uint4 u;
-        u.x = pack_bf16(p[0], p[1]);
-        u.y = pack_bf16(p[2], p[3]);
-        u.z = pack_bf16(p[4], p[5]);
-        u.w = pack_bf16(p[6], p[7]);
-        const int chunk = (g & 7) ^ (r & 7);
-        *reinterpret_cast<uint4*>(p_row + (g >> 3) * (ATT_BQ * 128) + chunk * 16) = u;
+      for (int i = 0; i < 16; ++i) {
+        mx[0] = fmaxf(mx[0], fmaxf(sv[4 * i], sv[4 * i + 1]));
+        mx[1] = fmaxf(mx[1], fmaxf(sv[4 * i + 2], sv[4 * i + 3]));
       }
-      l += rs;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_full);
-    }
-    // epilogue
-    mbar_wait(o_done, (n_kv - 1) & 1);
-    tc_fence_after();
-    const float inv = 1.f / l;
-    const bool row_ok = q_idx < Sq;
-    bf16* o_row = out + ((long long)seq * Sq + q_idx) * ld_out + head * D;
-#pragma unroll 1
-    for (int ch = 0; ch < D / 32; ++ch) {
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(tmem_O + lane_off + ch * 32, v);
-      tmem_wait_ld();
-      if (row_ok) {
+      float alpha[2], neg_m[2];
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 u;
-          u.x = pack_bf16(__uint_as_float(v[g * 8 + 0]) * inv, __uint_as_float(v[g * 8 + 1]) * inv);
-          u.y = pack_bf16(__uint_as_float(v[g * 8 + 2]) * inv, __uint_as_float(v[g * 8 + 3]) * inv);
-          u.z = pack_bf16(__uint_as_float(v[g * 8 + 4]) * inv, __uint_as_float(v[g * 8 + 5]) * inv);
-          u.w = pack_bf16(__uint_as_float(v[g * 8 + 6]) * inv, __uint_as_float(v[g * 8 + 7]) * inv);
-          *reinterpret_cast<uint4*>(o_row + ch * 32 + g * 8) = u;
-        }
-      }
-    }
-    if (row_ok && lse_out)
-      lse_out[((long long)seq * n_heads + head) * Sq + q_idx] = (m_used + log2f(l)) * LN2;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-}
-
-// ================================================================================================
-// forward, ping-pong form (default): one CTA owns TWO adjacent 128-row query tiles (A, B) of one (sequence, head) and
-// shares their K/V stream. While the 128 softmax threads of tile A work on S_A, the tensor pipe runs the MMAs of tile B
-// and vice versa, so neither unit waits for the other any more (the single-tile kernel above is a strict
-// MMA -> softmax -> MMA chain: sm__pipe_tensor_cycles_active 21 %).
-//   warps 0-3  softmax / epilogue of tile A (thread = query row = TMEM lane)
-//   warps 4-7  softmax / epilogue of tile B
-//   warp  8    TMA producer (Q_A, Q_B once; K/V ring)
-//   warp  9    MMA issuer, TMEM owner            (warps 10-11 only complete the third warpgroup)
-// Register budget: the producer warpgroup gives its registers back (setmaxnreg.dec 56) and the two softmax warpgroups
-// take 224 each (8*32*224 + 4*32*56 = 64512 = the 168 x 384 registers the CTA was launched with), so the 128-column row stays in registers with room to pipeline.
-// TMEM (512 columns): S_A [0,128) S_B [128,256) O_A [256,256+D) O_B [384,384+D). P = exp2(S - m) is written back
-// as packed bf16 into the first 64 columns of its own S buffer and consumed from there as the A operand of the PV MMA
-// (tcgen05.mma with A in TMEM) — no shared-memory round trip, no proxy fence. The next S MMA of the same tile is issued
-// after that PV (same issuing thread => pipeline order), which is what makes the aliasing safe.
-// ================================================================================================
-template <int D>
-struct AttFwd2Cfg {
-  static constexpr int STAGES = (D == 128) ? 2 : 4;
-  static constexpr uint32_t Q_BYTES = ATT_BQ * D * 2;
-  static constexpr uint32_t KV_BYTES = ATT_BKV * D * 2;   // one of K or V
-  static constexpr uint32_t OFF_Q = 0;                      // [2]
-  static constexpr uint32_t OFF_K = 2 * Q_BYTES;            // [STAGES]
-  static constexpr uint32_t OFF_V = OFF_K + STAGES * KV_BYTES;
-  static constexpr uint32_t OFF_BAR = OFF_V + STAGES * KV_BYTES;
-  static constexpr uint32_t SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static constexpr uint32_t TMEM_COLS = 512;
-};
-
-template <int D, bool CAUSAL>
-__global__ void __launch_bounds__(384, 1)
-attention_fwd2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                      const __grid_constant__ CUtensorMap tmV, bf16* __restrict__ out, long long ld_out,
-                      float* __restrict__ lse_out, int Sq, int Skv, int n_heads, int kv_group, int q_shared,
-                      float scale) {
-  using Cfg = AttFwd2Cfg<D>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* q_full = bars + 0;               // [2]
-  uint64_t* kv_full = bars + 2;              // [STAGES]
-  uint64_t* kv_empty = bars + 2 + STAGES;    // [STAGES]
-  uint64_t* s_full = bars + 2 + 2 * STAGES;  // [2]
-  uint64_t* p_full = s_full + 2;             // [2]
-  uint64_t* o_final = p_full + 2;            // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_final + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_q_tiles = (Sq + ATT_BQ - 1) / ATT_BQ;
-  const int pair = (int)gridDim.x - 1 - (int)blockIdx.x;   // heavy (late) tiles first
-  const int qt[2] = {2 * pair, 2 * pair + 1};
-  const bool has_b = qt[1] < num_q_tiles;
-  const int head = blockIdx.y, seq = blockIdx.z;
-  const int q_seq = q_shared ? 0 : seq;
-  const int kv_head = head / kv_group;
-  const int n_kv_all = (Skv + ATT_BKV - 1) / ATT_BKV;
-  const int n_of[2] = {CAUSAL ? qt[0] + 1 : n_kv_all, has_b ? (CAUSAL ? qt[1] + 1 : n_kv_all) : 0};
-  const int n_kv = n_of[0] > n_of[1] ? n_of[0] : n_of[1];
-
-  // The producer thread initialises the barriers its loads complete on and issues the Q tiles and the first K/V
-  // stages before the CTA-wide sync: TMEM allocation and the other barriers overlap the load latency.
-  auto load_kv = [&](int j) {
-    const int s = j % STAGES;
-    mbar_arrive_expect_tx(&kv_full[s], 2 * Cfg::KV_BYTES);
-#pragma unroll
-    for (int a = 0; a < D / 64; ++a) {
-      tma_load_3d(smem + Cfg::OFF_K + s * Cfg::KV_BYTES + a * (ATT_BKV * 128), &tmK, &kv_full[s], kv_head * D + a * 64,
-                  j * ATT_BKV, seq);
-      tma_load_3d(smem + Cfg::OFF_V + s * Cfg::KV_BYTES + a * (ATT_BKV * 128), &tmV, &kv_full[s], kv_head * D + a * 64,
-                  j * ATT_BKV, seq);
-    }
-  };
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    for (int i = 0; i < 2; ++i) mbar_init(&q_full[i], 1);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-    fence_barrier_init();
-    for (int x = 0; x < 2; ++x) {
-      if (x == 1 && !has_b) break;
-      mbar_arrive_expect_tx(&q_full[x], Cfg::Q_BYTES);
-#pragma unroll
-      for (int a = 0; a < D / 64; ++a)
-        tma_load_3d(smem + Cfg::OFF_Q + x * Cfg::Q_BYTES + a * (ATT_BQ * 128), &tmQ, &q_full[x], head * D + a * 64,
-                    qt[x] * ATT_BQ, q_seq);
-    }
-    for (int j = 0; j < n_kv && j < STAGES; ++j) load_kv(j);
-  }
-  if (warp == 9) {
-    if (lane == 0) {
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&s_full[i], 1);
-        mbar_init(&p_full[i], 128);
-        mbar_init(&o_final[i], 1);
-      }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp >= 8) {
-   setmaxnreg_dec<56>();      // inside the role branch: ptxas budgets registers per region from here on
-   if (warp == 8) {
-    // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
-      for (int j = STAGES; j < n_kv; ++j) {          // the first STAGES tiles were issued before the CTA sync
-        mbar_wait(&kv_empty[j % STAGES], ((j / STAGES) - 1) & 1);
-        load_kv(j);
-      }
-    }
-  } else if (warp == 9) {
-    // ------------------------------ MMA issuer ------------------------------
-    // The WHOLE warp runs this loop (uniform control flow, so descriptors and addresses live in uniform registers)
-    // and one elected lane issues each tcgen05 instruction. With `if (lane == 0)` around the loop every operand went
-    // through R2UR moves and ~100 cycles of single-thread address arithmetic per MMA — longer than the 64-cycle MMA.
-    {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, ATT_BKV, false, false);
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, D, false, true);
-      const bool leader = elect_one();
-      int kv_ready = 0;                      // K/V stages 0 .. kv_ready-1 have been waited for
-      auto need_kv = [&](int j) {
-        while (kv_ready <= j) {
-          mbar_wait(&kv_full[kv_ready % STAGES], (kv_ready / STAGES) & 1);
-          ++kv_ready;
-        }
-        tc_fence_after();
-      };
-      auto issue_s = [&](int x, int j) {
-        need_kv(j);
-        const uint32_t q_addr = smem_u32(smem + Cfg::OFF_Q + x * Cfg::Q_BYTES);
-        const uint32_t k_addr = smem_u32(smem + Cfg::OFF_K + (j % STAGES) * Cfg::KV_BYTES);
-        const uint64_t qd = desc_kmajor(q_addr, 0), kd = desc_kmajor(k_addr, 0);
-        if (leader) {
-#pragma unroll
-          for (int k16 = 0; k16 < D / 16; ++k16) {
-            // start-address field counts 16-byte units: +2 per 32-byte K step, +(rows*128/16) per 64-column atom
-            const uint64_t off = (uint64_t)((k16 >> 2) * (ATT_BQ * 128 / 16) + (k16 & 3) * 2);
-            umma_ss(tmem_base + x * 128, qd + off, kd + off, idesc_s, k16 > 0 ? 1u : 0u);
-          }
-          umma_commit(&s_full[x]);
-        }
-        __syncwarp();
-      };
-      auto issue_pv = [&](int x, int j) {
-        const uint32_t v_addr = smem_u32(smem + Cfg::OFF_V + (j % STAGES) * Cfg::KV_BYTES);
-        const uint64_t vd = desc_mnmajor(v_addr, 0, ATT_BKV);
-        if (leader) {
-#pragma unroll
-          for (int k16 = 0; k16 < ATT_BKV / 16; ++k16) {
-            // A = P (bf16 pairs, 8 TMEM columns per 16 kv), B = V tile read MN-major (+2048 bytes per 16 kv rows)
-            umma_ts(tmem_base + 256 + x * 128, tmem_base + x * 128 + k16 * 8, vd + (uint64_t)(k16 * (2048 / 16)),
-                    idesc_o, (j > 0 || k16 > 0) ? 1u : 0u);
-          }
-        }
-        __syncwarp();
-      };
-      mbar_wait(&q_full[0], 0);
-      if (has_b) mbar_wait(&q_full[1], 0);
-      issue_s(0, 0);
-      if (has_b) issue_s(1, 0);
-      for (int j = 0; j < n_kv; ++j) {
-        for (int x = 0; x < 2; ++x) {
-          if (j >= n_of[x]) continue;
-          mbar_wait(&p_full[x], j & 1);
-          tc_fence_after();
-          issue_pv(x, j);
-          if (j + 1 < n_of[x]) issue_s(x, j + 1);
-          else if (leader) umma_commit(&o_final[x]);
-        }
-        if (leader) umma_commit(&kv_empty[j % STAGES]);
-        __syncwarp();
-      }
-    }
-   }
-  } else {
-    // ------------------------------ softmax / epilogue: one thread per query row ------------------------------
-    setmaxnreg_inc<224>();
-    const int x = warp >> 2;                 // 0: tile A, 1: tile B
-    const int nx = n_of[x];
-    if (nx > 0) {
-      const int r = (warp & 3) * 32 + lane;  // row in tile == TMEM lane
-      const int q_idx = qt[x] * ATT_BQ + r;
-      const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;
-      const uint32_t tS = tmem_base + x * 128 + lane_off;
-      const uint32_t tO = tmem_base + 256 + x * 128 + lane_off;
-      const float c = scale * LOG2E;
-      float m_used = -INFINITY, l = 0.f;
-      for (int j = 0; j < nx; ++j) {
-        mbar_wait(&s_full[x], j & 1);
-        tc_fence_after();
-        const int kv0 = j * ATT_BKV;
-        const bool need_mask = (kv0 + ATT_BKV > Skv) || (CAUSAL && j == qt[x]);
-        uint32_t v[128];
-        tmem_ld_32x32b_x64(tS, v);
-        tmem_ld_32x32b_x64(tS + 64, v + 64);
-        tmem_wait_ld();
-        if (need_mask) {
-#pragma unroll
-          for (int i = 0; i < 128; ++i) {
-            const int kv = kv0 + i;
-            if ((kv >= Skv) || (CAUSAL && kv > q_idx)) v[i] = 0xff800000u;   // -inf
-          }
-        }
-        // row max: four independent chains (the serial 128-deep FMNMX chain was latency, not throughput)
-        float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-        for (int i = 0; i < 128; i += 4) {
-          mx4[0] = fmaxf(mx4[0], __uint_as_float(v[i]));
-          mx4[1] = fmaxf(mx4[1], __uint_as_float(v[i + 1]));
-          mx4[2] = fmaxf(mx4[2], __uint_as_float(v[i + 2]));
-          mx4[3] = fmaxf(mx4[3], __uint_as_float(v[i + 3]));
-        }
-        const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-        float m_new = fmaxf(m_used, mx * c);
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        float m_new = fmaxf(m_run[h], mx[h] * c);
         if (m_new == -INFINITY) m_new = 0.f;
-        if (j == 0) {
-          m_used = m_new;
-        } else {
-          // S_x(j) is complete => PV_x(j-1), issued before it by the same thread, is complete too: O is readable
-          const bool need = (m_new - m_used) > 8.0f;
-          if (__any_sync(0xffffffffu, need)) {
-            const float alpha = need ? fast_exp2(m_used - m_new) : 1.f;
-            if (need) { m_used = m_new; l *= alpha; }
-#pragma unroll 1
-            for (int ch = 0; ch < D / 32; ++ch) {
-              uint32_t o[32];
-              tmem_ld_32x32b_x32(tO + ch * 32, o);
-              tmem_wait_ld();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-              tmem_st_32x32b_x32(tO + ch * 32, o);
-            }
-          }
-        }
-        // P = exp2(s*c - m) -> packed bf16 pairs -> the first 64 columns of this tile's S buffer.
-        // Explicit phases over the register-resident row (in place, no extra registers): all FFMAs, then all MUFU.EX2
-        // back to back (the XU pipe is the scarce unit: keep it streaming), then sums on four accumulators + packing.
-        const float neg_m = -m_used;
-#pragma unroll
-        for (int i = 0; i < 128; ++i) v[i] = __float_as_uint(fmaf(__uint_as_float(v[i]), c, neg_m));
-#pragma unroll
-        for (int i = 0; i < 128; ++i) v[i] = __float_as_uint(fast_exp2(__uint_as_float(v[i])));   // exp2(-inf) = 0
-        float rs4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float p0 = __uint_as_float(v[g * 32 + 2 * i]), p1 = __uint_as_float(v[g * 32 + 2 * i + 1]);
-            rs4[i & 3] += p0 + p1;
-            pk[i] = pack_bf16(p0, p1);
-          }
-          tmem_st_32x32b_x16(tS + g * 16, pk);
-        }
-        const float rs = (rs4[0] + rs4[1]) + (rs4[2] + rs4[3]);
-        l += rs;
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&p_full[x]);
+        // the running max is only raised once it has grown by more than 8 (P <= 2^8 stays exact in fp32 and in the
+        // bf16 exponent range): fewer O rescales, and P's bf16 rounding follows the bf16 reference more closely on long
+        // sequences (DPO loss of the long tiny-model fixture: 1.7e-4 from the bf16 reference, 1.3e-3 with an eagerly
+        // updated max)
+        if (j > 0 && m_new - m_run[h] <= 8.0f) m_new = m_run[h];
+        alpha[h] = fast_exp2(m_run[h] - m_new);      // 0 on the first tile (m_run = -inf)
+        m_run[h] = m_new;
+        l[h] *= alpha[h];
+        neg_m[h] = -m_new;
       }
-      // epilogue: O / l -> bf16, staged through this tile's Q buffer (its last S MMA is complete once o_final fires)
-      mbar_wait(&o_final[x], 0);
-      tc_fence_after();
-      const float inv = 1.f / l;
-      const bool row_ok = q_idx < Sq;
-      {
-        const int wq = warp & 3;
-        const int row0 = qt[x] * ATT_BQ + wq * 32;                        // first query row of this warp
-        uint8_t* stage = smem + Cfg::OFF_Q + x * Cfg::Q_BYTES + wq * (32 * D * 2);
-        store_tile_rows<D / 32>(tO, inv, stage, lane, out + ((long long)seq * Sq + row0) * ld_out + head * D, ld_out,
-                                Sq - row0);
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i) {
+        o[4 * i] *= alpha[0]; o[4 * i + 1] *= alpha[0];
+        o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
       }
-      if (row_ok && lse_out)
-        lse_out[((long long)seq * n_heads + head) * Sq + q_idx] = (m_used + log2f(l)) * LN2;
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float p = fast_exp2(fmaf(sv[4 * i + e], c, neg_m[e >> 1]));   // exp2(-inf) = 0 for masked
+          sv[4 * i + e] = p;
+          l[e >> 1] += p;
+        }
+      uint32_t pa[8][4];
+      acc_to_afrag<8>(sv, pa);
+      reg_fence(o);
+      wgmma_fence();
+      mma_pv<D, 8>(o, pa, v_addr, Cfg::KV_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
+      if (lane == 0) mbar_arrive(&kv_empty[s]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+    // epilogue: O / l -> bf16, LSE
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+      const int q = qr[h];
+      if (q >= Sq) continue;
+      const float inv = 1.f / l[h];
+      bf16* o_row = out + ((long long)seq * Sq + q) * ld_out + head * D + fp.c0;
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i)
+        *reinterpret_cast<uint32_t*>(o_row + 8 * i) = pack_bf16(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+      if (lse_out && fp.c0 == 0) lse_out[((long long)seq * n_heads + head) * Sq + q] = (m_run[h] + log2f(l[h])) * LN2;
+    }
   }
 }
 
@@ -650,716 +299,294 @@ __global__ void attention_delta_kernel(const bf16* __restrict__ o, long long ld_
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// dK / dV: one CTA per (128-row K/V tile, kv head, sequence); math warpgroup wg owns kv rows [64*wg, 64*wg + 64).
+// Two passes over every (query head of the kv group, 64-row chunk of Q / dO), streamed through a two-stage TMA ring:
+//   pass 0 (dV): S^T = K Q^T, P^T = exp2(S^T*c - lse), dV += bf16(P^T) dO
+//   pass 1 (dK): S^T, dP^T = V dO^T, dS^T = P^T (dP^T - delta) * scale, dK += bf16(dS^T) Q
+// with the A operands straight from registers. One 64 x 128 fp32 accumulator is live at a time: dK and dV together
+// with S^T and dP^T do not fit the 168 registers a thread of this CTA has; the price is one more K Q^T per chunk.
+// q_shared: Q belongs to sequence 0 for every image (the resampler's learned queries).
+// ------------------------------------------------------------------------------------------------
+constexpr int BWD_D = 128;
+constexpr int BWD_C = 64;                                      // rows per streamed chunk
 struct AttBwdCfg {
-  static constexpr int D = 128;
-  static constexpr uint32_t TILE_BYTES = 128 * 128 * 2;  // 32 KB: any [128 x 128] bf16 tile
-  static constexpr uint32_t OFF_K = 0;
-  static constexpr uint32_t OFF_V = TILE_BYTES;
-  static constexpr uint32_t OFF_Q = 2 * TILE_BYTES;
-  static constexpr uint32_t OFF_DO = 3 * TILE_BYTES;
-  static constexpr uint32_t OFF_PT = 4 * TILE_BYTES;
-  static constexpr uint32_t OFF_DST = 5 * TILE_BYTES;
-  static constexpr uint32_t OFF_LSE = 6 * TILE_BYTES;         // 128 floats
-  static constexpr uint32_t OFF_DELTA = OFF_LSE + 512;        // 128 floats
-  static constexpr uint32_t OFF_BAR = OFF_DELTA + 512;
+  static constexpr uint32_t TILE_ATOM = 128 * 128;             // resident [128 rows][64 cols] atom
+  static constexpr uint32_t TILE_BYTES = 128 * BWD_D * 2;
+  static constexpr uint32_t CHUNK_ATOM = BWD_C * 128;          // streamed [64 rows][64 cols] atom
+  static constexpr uint32_t CHUNK_BYTES = BWD_C * BWD_D * 2;
+  static constexpr uint32_t OFF_T1 = TILE_BYTES;               // second resident tile
+  static constexpr uint32_t OFF_C = 2 * TILE_BYTES;            // [STAGES][2 chunks]
+  static constexpr uint32_t OFF_BAR = OFF_C + ATT_STAGES * 2 * CHUNK_BYTES;
   static constexpr uint32_t SMEM_BYTES = OFF_BAR + 128 + 1024;
-  static constexpr uint32_t TMEM_COLS = 512;  // S^T/dQ [0,128) dP^T [128,256) dV [256,384) dK [384,512)
 };
 
-// One CTA per (kv tile, head, seq). Thread r of warps 0..3 owns kv row r of the tile (TMEM lane r).
-__global__ void __launch_bounds__(160, 1)
-attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                     const float* __restrict__ lse, const float* __restrict__ delta,
-                     float* __restrict__ dq_f32, bf16* __restrict__ dk, bf16* __restrict__ dv,
-                     long long ld_dkv, int Sq, int Skv, int n_heads, int kv_group, int causal, int q_shared,
-                     float scale) {
-  // grid.y = key/value heads; the CTA loops over the kv_group query heads that share its K/V tile.
-  // q_shared: Q (and the dQ accumulator) belong to sequence 0 for every image — the fp32 red.add then also
-  // sums dQ over the batch, which is the gradient of the resampler's shared learned queries.
+template <bool DK>
+__device__ __forceinline__ void dkv_pass(uint8_t* smem, uint64_t* c_full, uint64_t* c_empty, int it0, int n_it, int n_c,
+                                         int c_first, int kv_head, int kv_group, int seq, int Sq, int n_heads,
+                                         int causal, const int (&kvr)[2], uint32_t k_addr, uint32_t v_addr, float c,
+                                         float scale, const float* __restrict__ lse, const float* __restrict__ delta,
+                                         float (&acc)[BWD_D / 2]) {
   using Cfg = AttBwdCfg;
-  constexpr int D = Cfg::D;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* kv_full = bars + 0;
-  uint64_t* q_full = bars + 1;    // Q_i, dO_i landed
-  uint64_t* st_full = bars + 2;   // S^T and dP^T MMAs done
-  uint64_t* pt_full = bars + 3;   // P^T, dS^T written to smem (128 arrivals)
-  uint64_t* acc_done = bars + 4;  // dV, dK, dQ MMAs of this iteration done
-  uint64_t* dq_read = bars + 5;   // dQ tile drained from TMEM (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
-  float* s_lse = reinterpret_cast<float*>(smem + Cfg::OFF_LSE);
-  float* s_delta = reinterpret_cast<float*>(smem + Cfg::OFF_DELTA);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_q_tiles = (Sq + 127) / 128;
-  const int kv_tile = blockIdx.x;
-  const int kv_head = blockIdx.y, seq = blockIdx.z;
-  const int q_seq = q_shared ? 0 : seq;
-  const int kv0 = kv_tile * 128;
-  const int q_first = causal ? kv_tile : 0;  // causal: q tiles kv_tile .. last (per query head); else all
-  const int n_qt = num_q_tiles - q_first;
-  const int n_q = n_qt * kv_group;           // iterations: (query head of the group) x (q tile)
-
-  if (warp == 4) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
-      mbar_init(kv_full, 1);
-      mbar_init(q_full, 1);
-      mbar_init(st_full, 1);
-      mbar_init(pt_full, 128);
-      mbar_init(acc_done, 1);
-      mbar_init(dq_read, 128);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_ST = tmem_base, tmem_DPT = tmem_base + 128, tmem_DV = tmem_base + 256,
-                 tmem_DK = tmem_base + 384, tmem_DQ = tmem_base;  // dQ reuses the S^T columns
-
-  const uint32_t k_addr = smem_u32(smem + Cfg::OFF_K), v_addr = smem_u32(smem + Cfg::OFF_V);
-  const uint32_t q_addr = smem_u32(smem + Cfg::OFF_Q), do_addr = smem_u32(smem + Cfg::OFF_DO);
-  const uint32_t pt_addr = smem_u32(smem + Cfg::OFF_PT), dst_addr = smem_u32(smem + Cfg::OFF_DST);
-
-  if (warp == 4) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_kk = make_idesc_bf16(128, 128, false, false);  // both K-major
-      constexpr uint32_t idesc_kmn = make_idesc_bf16(128, 128, false, true);  // A K-major, B MN-major
-      constexpr uint32_t idesc_mnmn = make_idesc_bf16(128, 128, true, true);  // both MN-major
-      mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
-      for (int a = 0; a < 2; ++a) {
-        tma_load_3d(smem + Cfg::OFF_K + a * 16384, &tmK, kv_full, kv_head * D + a * 64, kv0, seq);
-        tma_load_3d(smem + Cfg::OFF_V + a * 16384, &tmV, kv_full, kv_head * D + a * 64, kv0, seq);
+  const FragPos fp = frag_pos();
+#pragma unroll
+  for (int i = 0; i < BWD_D / 2; ++i) acc[i] = 0.f;
+  for (int it = 0; it < n_it; ++it) {
+    const int ii = it0 + it, s = ii % ATT_STAGES;
+    const int qc0 = (c_first + it % n_c) * BWD_C;
+    const int head = kv_head * kv_group + it / n_c;
+    const long long base = ((long long)seq * n_heads + head) * Sq;
+    const uint32_t q_addr = smem_u32(smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES);
+    const uint32_t do_addr = q_addr + Cfg::CHUNK_BYTES;
+    mbar_wait(&c_full[s], (ii / ATT_STAGES) & 1);
+    float st[32], dpt[32];
+    wgmma_fence();
+    mma_qk_64<BWD_D>(st, k_addr, Cfg::TILE_ATOM, q_addr, Cfg::CHUNK_ATOM);
+    if (DK) mma_qk_64<BWD_D>(dpt, v_addr, Cfg::TILE_ATOM, do_addr, Cfg::CHUNK_ATOM);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(st);
+    if (DK) reg_fence(dpt);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int q = qc0 + 8 * i + fp.c0;
+      // padded q: lse = +inf => P = 0
+      const float l0 = q < Sq ? lse[base + q] * LOG2E : INFINITY, l1 = q + 1 < Sq ? lse[base + q + 1] * LOG2E : INFINITY;
+      float d0 = 0.f, d1 = 0.f;
+      if (DK) {
+        d0 = q < Sq ? delta[base + q] : 0.f;
+        d1 = q + 1 < Sq ? delta[base + q + 1] : 0.f;
       }
-      auto load_q = [&](int it) {
-        const int q0 = (q_first + it % n_qt) * 128;
-        const int head = kv_head * kv_group + it / n_qt;
-        mbar_arrive_expect_tx(q_full, 2 * Cfg::TILE_BYTES);
-        for (int a = 0; a < 2; ++a) {
-          tma_load_3d(smem + Cfg::OFF_Q + a * 16384, &tmQ, q_full, head * D + a * 64, q0, q_seq);
-          tma_load_3d(smem + Cfg::OFF_DO + a * 16384, &tmDO, q_full, head * D + a * 64, q0, seq);
-        }
-      };
-      load_q(0);
-      mbar_wait(kv_full, 0);
-      for (int it = 0; it < n_q; ++it) {
-        mbar_wait(q_full, it & 1);
-        if (it > 0) mbar_wait(dq_read, (it - 1) & 1);  // dQ columns (== S^T columns) drained
-        tc_fence_after();
-        // S^T[kv][q] = K Q^T ; dP^T[kv][q] = V dO^T   (contraction over d, all K-major)
 #pragma unroll
-        for (int k16 = 0; k16 < 8; ++k16) {
-          umma_ss(tmem_ST, desc_kmajor(k_addr + (k16 >> 2) * 16384, k16 & 3),
-                  desc_kmajor(q_addr + (k16 >> 2) * 16384, k16 & 3), idesc_kk, k16 > 0);
-        }
-#pragma unroll
-        for (int k16 = 0; k16 < 8; ++k16) {
-          umma_ss(tmem_DPT, desc_kmajor(v_addr + (k16 >> 2) * 16384, k16 & 3),
-                  desc_kmajor(do_addr + (k16 >> 2) * 16384, k16 & 3), idesc_kk, k16 > 0);
-        }
-        umma_commit(st_full);
-        mbar_wait(pt_full, it & 1);
-        tc_fence_after();
-        // dV[kv][d] += P^T[kv][q] dO[q][d]   (A = P^T K-major over q, B = dO tile read MN-major)
-        // dK[kv][d] += dS^T[kv][q] Q[q][d]
-#pragma unroll
-        for (int k16 = 0; k16 < 8; ++k16) {
-          umma_ss(tmem_DV, desc_kmajor(pt_addr + (k16 >> 2) * 16384, k16 & 3),
-                  desc_mnmajor(do_addr, k16, 128), idesc_kmn, (it > 0 || k16 > 0));
-        }
-#pragma unroll
-        for (int k16 = 0; k16 < 8; ++k16) {
-          umma_ss(tmem_DK, desc_kmajor(dst_addr + (k16 >> 2) * 16384, k16 & 3),
-                  desc_mnmajor(q_addr, k16, 128), idesc_kmn, (it > 0 || k16 > 0));
-        }
-        // dQ[q][d] = dS[q][kv] K[kv][d]  (A = dS^T tile read MN-major: M=q contiguous; B = K tile MN-major)
-#pragma unroll
-        for (int k16 = 0; k16 < 8; ++k16) {
-          umma_ss(tmem_DQ, desc_mnmajor(dst_addr, k16, 128), desc_mnmajor(k_addr, k16, 128), idesc_mnmn,
-                  k16 > 0);
-        }
-        umma_commit(acc_done);
-        if (it + 1 < n_q) {
-          mbar_wait(acc_done, it & 1);  // Q/dO smem free again
-          load_q(it + 1);
-        }
+      for (int e = 0; e < 4; ++e) {
+        const int qq = q + (e & 1);
+        const bool masked = causal && kvr[e >> 1] > qq;
+        const float p = masked ? 0.f : fast_exp2(st[4 * i + e] * c - ((e & 1) ? l1 : l0));
+        st[4 * i + e] = DK ? p * (dpt[4 * i + e] - ((e & 1) ? d1 : d0)) * scale : p;
       }
     }
-  } else {
-    const int r = warp * 32 + lane;  // kv row within tile, TMEM lane; also q row for the dQ drain
-    const int kv_idx = kv0 + r;
-    const uint32_t lane_off = (uint32_t)(warp * 32) << 16;
-    const float c = scale * LOG2E;
-    for (int it = 0; it < n_q; ++it) {
-      const int q_tile = q_first + it % n_qt;
-      const int head = kv_head * kv_group + it / n_qt;
-      const int q0 = q_tile * 128;
-      // stage LSE / delta of this q tile (previous readers finished before last pt_full arrive;
-      // named barrier among the 128 compute threads keeps it simple)
-      asm volatile("bar.sync 1, 128;");
-      {
-        const int q = q0 + r;
-        const long long base = ((long long)seq * n_heads + head) * Sq;
-        s_lse[r] = q < Sq ? lse[base + q] * LOG2E : INFINITY;   // exp2(x - inf) = 0 for padded q
-        s_delta[r] = q < Sq ? delta[base + q] : 0.f;
-      }
-      asm volatile("bar.sync 1, 128;");
-      mbar_wait(st_full, it & 1);
-      tc_fence_after();
-      const bool diag = causal && (q_tile == kv_tile);
-      uint8_t* pt_row = smem + Cfg::OFF_PT + r * 128;
-      uint8_t* dst_row = smem + Cfg::OFF_DST + r * 128;
-#pragma unroll 1
-      for (int hf = 0; hf < 2; ++hf) {
-        uint32_t sv[64], dpv[64];
-        tmem_ld_32x32b_x64(tmem_ST + lane_off + hf * 64, sv);
-        tmem_ld_32x32b_x64(tmem_DPT + lane_off + hf * 64, dpv);
-        tmem_wait_ld();
-        uint8_t* pb = pt_row + hf * 16384;
-        uint8_t* db = dst_row + hf * 16384;
-#pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          float p[8], ds[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int qi = hf * 64 + g * 8 + i;
-            const bool masked = (kv_idx >= Skv) || (diag && kv_idx > q0 + qi);
-            const float pv = masked ? 0.f : fast_exp2(__uint_as_float(sv[g * 8 + i]) * c - s_lse[qi]);
-            p[i] = pv;
-            ds[i] = pv * (__uint_as_float(dpv[g * 8 + i]) - s_delta[qi]) * scale;
-          }
-          const int chunk = g ^ (r & 7);
-          uint4 u, w;
-          u.x = pack_bf16(p[0], p[1]); u.y = pack_bf16(p[2], p[3]);
-          u.z = pack_bf16(p[4], p[5]); u.w = pack_bf16(p[6], p[7]);
-          w.x = pack_bf16(ds[0], ds[1]); w.y = pack_bf16(ds[2], ds[3]);
-          w.z = pack_bf16(ds[4], ds[5]); w.w = pack_bf16(ds[6], ds[7]);
-          *reinterpret_cast<uint4*>(pb + chunk * 16) = u;
-          *reinterpret_cast<uint4*>(db + chunk * 16) = w;
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(pt_full);
-      // drain dQ tile: TMEM lane r = q row q0 + r
-      mbar_wait(acc_done, it & 1);
-      tc_fence_after();
-      {
-        const int q = q0 + r;
-        float* dq_row = dq_f32 + ((long long)q_seq * Sq + q) * ((long long)n_heads * D) + head * D;
-#pragma unroll 1
-        for (int ch = 0; ch < 4; ++ch) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(tmem_DQ + lane_off + ch * 32, v);
-          tmem_wait_ld();
-          if (q < Sq) {
-            // 128-bit vector reductions: 4x fewer L2 atomic operations than scalar red.add
-#pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dq_row + ch * 32 + i),
-                           "f"(__uint_as_float(v[i])), "f"(__uint_as_float(v[i + 1])),
-                           "f"(__uint_as_float(v[i + 2])), "f"(__uint_as_float(v[i + 3]))
-                           : "memory");
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(dq_read);
-    }
-    // epilogue: dV, dK rows (kv row r) -> bf16 global
-    // acc_done for the last iteration was already waited above
-    tc_fence_after();
-    {
-      const bool row_ok = kv_idx < Skv;  // loads stay warp-convergent; only the stores are predicated
-      bf16* dv_row = dv + ((long long)seq * Skv + kv_idx) * ld_dkv + kv_head * D;
-      bf16* dk_row = dk + ((long long)seq * Skv + kv_idx) * ld_dkv + kv_head * D;
-#pragma unroll 1
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t a[32], b[32];
-        tmem_ld_32x32b_x32(tmem_DV + lane_off + ch * 32, a);
-        tmem_ld_32x32b_x32(tmem_DK + lane_off + ch * 32, b);
-        tmem_wait_ld();
-        if (row_ok) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4 u, w;
-            u.x = pack_bf16(__uint_as_float(a[g * 8 + 0]), __uint_as_float(a[g * 8 + 1]));
-            u.y = pack_bf16(__uint_as_float(a[g * 8 + 2]), __uint_as_float(a[g * 8 + 3]));
-            u.z = pack_bf16(__uint_as_float(a[g * 8 + 4]), __uint_as_float(a[g * 8 + 5]));
-            u.w = pack_bf16(__uint_as_float(a[g * 8 + 6]), __uint_as_float(a[g * 8 + 7]));
-            w.x = pack_bf16(__uint_as_float(b[g * 8 + 0]), __uint_as_float(b[g * 8 + 1]));
-            w.y = pack_bf16(__uint_as_float(b[g * 8 + 2]), __uint_as_float(b[g * 8 + 3]));
-            w.z = pack_bf16(__uint_as_float(b[g * 8 + 4]), __uint_as_float(b[g * 8 + 5]));
-            w.w = pack_bf16(__uint_as_float(b[g * 8 + 6]), __uint_as_float(b[g * 8 + 7]));
-            *reinterpret_cast<uint4*>(dv_row + ch * 32 + g * 8) = u;
-            *reinterpret_cast<uint4*>(dk_row + ch * 32 + g * 8) = w;
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+    uint32_t fa[4][4];
+    acc_to_afrag<4>(st, fa);
+    reg_fence(acc);
+    wgmma_fence();
+    mma_pv<BWD_D, 4>(acc, fa, DK ? q_addr : do_addr, Cfg::CHUNK_ATOM);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&c_empty[s]);
   }
 }
 
-// ================================================================================================
-// backward, split form (default for self-attention): two kernels, no atomics, no fp32 dQ buffer.
-//   attention_bwd_dkv_kernel : one CTA per (128-row K/V tile, kv head, sequence); streams 64-row chunks of Q / dO;
-//                              dV += P^T dO and dK += dS^T Q accumulate in TMEM (4 MMAs per chunk).
-//   attention_bwd_dq_kernel  : one CTA per (128-row Q tile, head, sequence); streams 64-row chunks of K / V;
-//                              dQ += dS K accumulates in TMEM (3 MMAs per chunk) and is written once as bf16.
-// The fused round-1 kernel did 5 MMAs per tile pair but reduced dQ with 64 KB of fp32 red.global per pair, drained
-// through the same TMEM columns the next S^T needed: a strictly serial chain (tensor pipe 19 % active). Here the
-// recomputation of S / dP is paid twice (7 MMAs instead of 5) and everything else is pipelined:
-//   * S^T / dP^T (resp. S / dP) are 64-column chunks, double-buffered in TMEM, so the MMAs of chunk c+1 run while the
-//     compute threads turn chunk c into P / dS;
-//   * two compute warpgroups take alternate chunks;
-//   * P^T and dS^T (resp. dS) go back into the TMEM columns they came from as packed bf16 and are consumed from there
-//     as the A operand (tcgen05.mma with A in TMEM): no shared-memory staging, no proxy fence;
-//   * warps 0-3 / 4-7 = compute groups, warp 8 = TMA, warp 9 = MMA issuer; setmaxnreg moves registers to the groups.
-// ================================================================================================
-struct AttBwd2Cfg {
-  static constexpr int D = 128;
-  static constexpr int CH = 64;                                   // rows per streamed chunk
-  static constexpr int STAGES = 4;
-  static constexpr uint32_t TILE_BYTES = 128 * D * 2;             // resident [128 x 128] tile
-  static constexpr uint32_t CHUNK_BYTES = CH * D * 2;             // streamed [64 x 128] chunk
-  static constexpr uint32_t OFF_RES0 = 0;                         // dkv: K   | dq: Q
-  static constexpr uint32_t OFF_RES1 = TILE_BYTES;                // dkv: V   | dq: dO
-  static constexpr uint32_t OFF_RING = 2 * TILE_BYTES;            // [STAGES][2 chunks]: dkv Q,dO | dq K,V
-  static constexpr uint32_t OFF_STAT = OFF_RING + STAGES * 2 * CHUNK_BYTES;   // dkv: [2 groups][2 buffers][lse 64 | delta 64] fp32
-  static constexpr uint32_t OFF_BAR = OFF_STAT + 2 * 2 * 2 * CH * 4;
-  static constexpr uint32_t SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static constexpr uint32_t TMEM_COLS = 512;
-};
-
-// K-major [rows x 128] tile made of two 64-column atoms of `rows` rows each
-__device__ __forceinline__ uint64_t desc_k_tile(uint32_t tile_addr, int k16, int rows) {
-  return desc_kmajor(tile_addr + (k16 >> 2) * (rows * 128), k16 & 3);
-}
-
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                          const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
                          const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dk,
                          bf16* __restrict__ dv, long long ld_dkv, int Sq, int Skv, int n_heads, int kv_group,
-                         int causal, float scale) {
-  using Cfg = AttBwd2Cfg;
-  constexpr int D = Cfg::D, CH = Cfg::CH, STAGES = Cfg::STAGES;
+                         int causal, int q_shared, float scale) {
+  using Cfg = AttBwdCfg;
+  constexpr int D = BWD_D;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* kv_full = bars + 0;
-  uint64_t* ring_full = bars + 1;                 // [STAGES]
-  uint64_t* ring_empty = bars + 1 + STAGES;       // [STAGES]
-  uint64_t* st_full = bars + 1 + 2 * STAGES;      // [2]  S^T / dP^T chunk ready
-  uint64_t* pt_full = st_full + 2;                // [2]  P^T / dS^T written (128 arrivals)
-  uint64_t* acc_done = pt_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_done + 1);
+  uint64_t* kv_full = bars;
+  uint64_t* c_full = bars + 1;                  // [STAGES]
+  uint64_t* c_empty = bars + 1 + ATT_STAGES;    // [STAGES]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kv_tile = blockIdx.x, kv_head = blockIdx.y, seq = blockIdx.z;
-  const int kv0 = kv_tile * 128;
-  const int q_begin = causal ? kv0 : 0;                            // first query row that can see this K/V tile
-  const int n_ch = (Sq - q_begin + CH - 1) / CH;                   // chunks per query head
-  const int n_it = n_ch * kv_group;
+  const int warp = threadIdx.x >> 5, wg = warp >> 2;
+  const int kv0 = blockIdx.x * 128;
+  const int kv_head = blockIdx.y, seq = blockIdx.z;
+  const int q_seq = q_shared ? 0 : seq;
+  const int n_chunks = (Sq + BWD_C - 1) / BWD_C;
+  const int c_first = causal ? kv0 / BWD_C : 0;               // causal: chunks holding a q >= kv0
+  const int n_c = n_chunks - c_first;
+  const int n_it = n_c > 0 ? n_c * kv_group : 0;               // (query head of the group) x (q chunk), per pass
 
-  // producer thread: own barriers, resident K / V tile and the first ring stages before the CTA-wide sync (see the dQ
-  // kernel)
-  auto load_chunk = [&](int it) {
-    const int s = it % STAGES;
-    const int head = kv_head * kv_group + it / n_ch;
-    const int q0 = q_begin + (it % n_ch) * CH;
-    uint8_t* dst = smem + Cfg::OFF_RING + s * 2 * Cfg::CHUNK_BYTES;
-    mbar_arrive_expect_tx(&ring_full[s], 2 * Cfg::CHUNK_BYTES);
-    for (int a = 0; a < 2; ++a) {
-      tma_load_3d(dst + a * (CH * 128), &tmQ, &ring_full[s], head * D + a * 64, q0, seq);
-      tma_load_3d(dst + Cfg::CHUNK_BYTES + a * (CH * 128), &tmDO, &ring_full[s], head * D + a * 64, q0, seq);
-    }
-  };
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
+  if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&ring_full[i], 1); mbar_init(&ring_empty[i], 1); }
+    for (int i = 0; i < ATT_STAGES; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 8); }
     fence_barrier_init();
-    mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
-    for (int a = 0; a < 2; ++a) {
-      tma_load_3d(smem + Cfg::OFF_RES0 + a * 16384, &tmK, kv_full, kv_head * D + a * 64, kv0, seq);
-      tma_load_3d(smem + Cfg::OFF_RES1 + a * 16384, &tmV, kv_full, kv_head * D + a * 64, kv0, seq);
-    }
-    for (int it = 0; it < n_it && it < STAGES; ++it) load_chunk(it);
   }
-  if (warp == 9) {
-    if (lane == 0) {
-      for (int i = 0; i < 2; ++i) { mbar_init(&st_full[i], 1); mbar_init(&pt_full[i], 128); }
-      mbar_init(acc_done, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // columns: S^T[b] = b*64, dP^T[b] = 128 + b*64, dV = 256, dK = 384
 
-  if (warp >= 8) {
-   setmaxnreg_dec<56>();
-   if (warp == 8) {
-    // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
-      for (int it = STAGES; it < n_it; ++it) {       // the first STAGES chunks were issued before the CTA sync
-        mbar_wait(&ring_empty[it % STAGES], ((it / STAGES) - 1) & 1);
-        load_chunk(it);
+  if (wg == 2) {
+    if (threadIdx.x == 256) {
+      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
+      mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
+      for (int a = 0; a < 2; ++a) {
+        tma_load_3d(smem + a * Cfg::TILE_ATOM, &tmK, kv_full, kv_head * D + a * 64, kv0, seq);
+        tma_load_3d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmV, kv_full, kv_head * D + a * 64, kv0, seq);
+      }
+      for (int ii = 0; ii < 2 * n_it; ++ii) {
+        const int it = ii % n_it, s = ii % ATT_STAGES;
+        if (ii >= ATT_STAGES) mbar_wait(&c_empty[s], ((ii / ATT_STAGES) - 1) & 1);
+        const int qc0 = (c_first + it % n_c) * BWD_C;
+        const int head = kv_head * kv_group + it / n_c;
+        uint8_t* dst = smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES;
+        mbar_arrive_expect_tx(&c_full[s], 2 * Cfg::CHUNK_BYTES);
+        for (int a = 0; a < 2; ++a) {
+          tma_load_3d(dst + a * Cfg::CHUNK_ATOM, &tmQ, &c_full[s], head * D + a * 64, qc0, q_seq);
+          tma_load_3d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmDO, &c_full[s], head * D + a * 64, qc0, seq);
+        }
       }
     }
-   } else if (warp == 9) {
-    // ------------------------------ MMA issuer (whole warp, elected lane issues) ------------------------------
-    {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, CH, false, false);    // [128 kv x 64 q] = K-major x K-major
-      constexpr uint32_t idesc_acc = make_idesc_bf16(128, D, false, true);    // A from TMEM, B = chunk read MN-major
-      const bool leader = elect_one();
-      const uint64_t kd = desc_kmajor(smem_u32(smem + Cfg::OFF_RES0), 0), vd = desc_kmajor(smem_u32(smem + Cfg::OFF_RES1), 0);
-      auto issue_s = [&](int it) {
-        const int s = it % STAGES, b = it & 1;
-        mbar_wait(&ring_full[s], (it / STAGES) & 1);
-        tc_fence_after();
-        const uint32_t q_addr = smem_u32(smem + Cfg::OFF_RING + s * 2 * Cfg::CHUNK_BYTES);
-        const uint64_t qd = desc_kmajor(q_addr, 0), dod = desc_kmajor(q_addr + Cfg::CHUNK_BYTES, 0);
-        if (leader) {
-#pragma unroll
-          for (int k16 = 0; k16 < D / 16; ++k16) {    // S^T = K Q^T   (16-byte units: +2 per K step, +rows*8 per atom)
-            const uint64_t oa = (uint64_t)((k16 >> 2) * (128 * 8) + (k16 & 3) * 2), ob = (uint64_t)((k16 >> 2) * (CH * 8) + (k16 & 3) * 2);
-            umma_ss(tmem_base + b * CH, kd + oa, qd + ob, idesc_s, k16 > 0);
-          }
-#pragma unroll
-          for (int k16 = 0; k16 < D / 16; ++k16) {    // dP^T = V dO^T
-            const uint64_t oa = (uint64_t)((k16 >> 2) * (128 * 8) + (k16 & 3) * 2), ob = (uint64_t)((k16 >> 2) * (CH * 8) + (k16 & 3) * 2);
-            umma_ss(tmem_base + 128 + b * CH, vd + oa, dod + ob, idesc_s, k16 > 0);
-          }
-          umma_commit(&st_full[b]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(kv_full, 0);
-      issue_s(0);
-      for (int it = 0; it < n_it; ++it) {
-        if (it + 1 < n_it) issue_s(it + 1);
-        const int s = it % STAGES, b = it & 1;
-        mbar_wait(&pt_full[b], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t q_addr = smem_u32(smem + Cfg::OFF_RING + s * 2 * Cfg::CHUNK_BYTES);
-        const uint64_t qm = desc_mnmajor(q_addr, 0, CH), dom = desc_mnmajor(q_addr + Cfg::CHUNK_BYTES, 0, CH);
-        if (leader) {
-#pragma unroll
-          for (int k16 = 0; k16 < CH / 16; ++k16)     // dV += P^T dO     (A = P^T: 8 TMEM columns per 16 q)
-            umma_ts(tmem_base + 256, tmem_base + b * CH + k16 * 8, dom + (uint64_t)(k16 * 128), idesc_acc,
-                    (it > 0 || k16 > 0));
-#pragma unroll
-          for (int k16 = 0; k16 < CH / 16; ++k16)     // dK += dS^T Q
-            umma_ts(tmem_base + 384, tmem_base + 128 + b * CH + k16 * 8, qm + (uint64_t)(k16 * 128), idesc_acc,
-                    (it > 0 || k16 > 0));
-          umma_commit(&ring_empty[s]);
-        }
-        __syncwarp();
-      }
-      if (leader) umma_commit(acc_done);
-      __syncwarp();
-    }
-   }
   } else {
-    // ------------------------------ compute groups: thread = kv row ------------------------------
-    setmaxnreg_inc<224>();
-    const int g = warp >> 2;                       // group g takes iterations it = g, g+2, ... (TMEM buffer b = g)
-    const int r = (warp & 3) * 32 + lane;
-    const int kv_idx = kv0 + r;
-    const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;
-    const uint32_t tST = tmem_base + g * CH + lane_off, tDPT = tmem_base + 128 + g * CH + lane_off;
-    float* s_stat = reinterpret_cast<float*>(smem + Cfg::OFF_STAT) + g * 4 * CH;   // [2 buffers][lse 64 | delta 64]
+    const FragPos fp = frag_pos();
+    const int kvr[2] = {kv0 + wg * 64 + fp.r0, kv0 + wg * 64 + fp.r0 + 8};
     const float c = scale * LOG2E;
-    const int tid_g = threadIdx.x & 127;
-    // lse (threads 0-63) / delta (64-127) of the 64 query rows of chunk `it`: loaded one chunk ahead into a register
-    // and parked in the other half of a double buffer at the end of the iteration, so the global-load latency is off
-    // the S^T -> P^T chain (it used to sit between two named barriers at the top of every iteration)
-    auto load_stat = [&](int it) -> float {
-      const int head = kv_head * kv_group + it / n_ch;
-      const int q = q_begin + (it % n_ch) * CH + (tid_g & 63);
-      const long long base = ((long long)seq * n_heads + head) * Sq;
-      if (q >= Sq) return tid_g < 64 ? INFINITY : 0.f;                      // exp2(x - inf) = 0 for padded rows
-      return tid_g < 64 ? lse[base + q] * LOG2E : delta[base + q];
-    };
-    if (g < n_it) s_stat[tid_g] = load_stat(g);
-    int k = 0;                                      // this group's iteration count: buffer k & 1
-    for (int it = g; it < n_it; it += 2, ++k) {
-      const int q0 = q_begin + (it % n_ch) * CH;
-      // one named barrier per iteration (ids 1, 2): publishes buffer k&1, and everyone is done reading buffer (k+1)&1
-      asm volatile("bar.sync %0, 128;" ::"r"(g + 1));
-      const float* s_lse = s_stat + (k & 1) * 2 * CH;
-      const float* s_delta = s_lse + CH;
-      const float next_stat = (it + 2 < n_it) ? load_stat(it + 2) : 0.f;
-      mbar_wait(&st_full[g], (it >> 1) & 1);
-      tc_fence_after();
-      uint32_t sv[64], dpv[64];
-      tmem_ld_32x32b_x64(tST, sv);
-      tmem_ld_32x32b_x64(tDPT, dpv);
-      tmem_wait_ld();
-      const bool diag = causal && (q0 < kv0 + 128);      // chunk overlaps the tile's diagonal block (uniform)
-      // masked keys (row beyond Skv, or above the causal diagonal) get s = -inf => p = exp2(-inf) = 0; the mask is a
-      // per-row column bound applied BEFORE the arithmetic, in a branch that only the diagonal chunks take
-      const int first_visible = kv_idx >= Skv ? 64 : (diag ? max(0, kv_idx - q0) : 0);   // columns < this are masked
-      if (first_visible > 0) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (i < first_visible) sv[i] = 0xff800000u;
-      }
-#pragma unroll
-      for (int i = 0; i < 64; ++i) {
-        const float pv = fast_exp2(fmaf(__uint_as_float(sv[i]), c, -s_lse[i]));
-        sv[i] = __float_as_uint(pv);
-        dpv[i] = __float_as_uint(pv * (__uint_as_float(dpv[i]) - s_delta[i]) * scale);
-      }
+    const uint32_t k_addr = smem_u32(smem) + wg * 64 * 128;
+    const uint32_t v_addr = smem_u32(smem + Cfg::OFF_T1) + wg * 64 * 128;
+    mbar_wait(kv_full, 0);
+    float acc[D / 2];
+#pragma unroll 1
+    for (int pass = 0; pass < 2; ++pass) {
+      if (pass == 0)
+        dkv_pass<false>(smem, c_full, c_empty, 0, n_it, n_c, c_first, kv_head, kv_group, seq, Sq, n_heads, causal, kvr,
+                        k_addr, v_addr, c, scale, lse, delta, acc);
+      else
+        dkv_pass<true>(smem, c_full, c_empty, n_it, n_it, n_c, c_first, kv_head, kv_group, seq, Sq, n_heads, causal, kvr,
+                       k_addr, v_addr, c, scale, lse, delta, acc);
+      bf16* dst = pass == 0 ? dv : dk;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        uint32_t pk[16], dk_[16];
+        const int kv = kvr[h];
+        if (kv >= Skv) continue;
+        bf16* row = dst + ((long long)seq * Skv + kv) * ld_dkv + kv_head * D + fp.c0;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          pk[i] = pack_bf16(__uint_as_float(sv[h * 32 + 2 * i]), __uint_as_float(sv[h * 32 + 2 * i + 1]));
-          dk_[i] = pack_bf16(__uint_as_float(dpv[h * 32 + 2 * i]), __uint_as_float(dpv[h * 32 + 2 * i + 1]));
-        }
-        tmem_st_32x32b_x16(tST + h * 16, pk);
-        tmem_st_32x32b_x16(tDPT + h * 16, dk_);
+        for (int i = 0; i < D / 8; ++i)
+          *reinterpret_cast<uint32_t*>(row + 8 * i) = pack_bf16(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
       }
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(&pt_full[g]);
-      s_stat[((k + 1) & 1) * 2 * CH + tid_g] = next_stat;
     }
-    // epilogue: group 0 stores dV, group 1 stores dK (kv row r)
-    mbar_wait(acc_done, 0);
-    tc_fence_after();
-    {
-      // every MMA is complete (acc_done), so the Q/dO ring is free: 8 KB of it per warp stages the coalesced stores
-      const int row0 = kv0 + (warp & 3) * 32;
-      uint8_t* stage = smem + Cfg::OFF_RING + warp * (32 * D * 2);
-      store_tile_rows<D / 32>(tmem_base + 256 + g * 128 + lane_off, 1.f, stage, lane,
-                              (g == 0 ? dv : dk) + ((long long)seq * Skv + row0) * ld_dkv + kv_head * D, ld_dkv,
-                              Skv - row0);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
-__global__ void __launch_bounds__(384, 1)
+// ------------------------------------------------------------------------------------------------
+// dQ: one CTA per (128-row Q tile, head, sequence); math warpgroup wg owns q rows [64*wg, 64*wg + 64). For every
+// 64-row chunk of K / V: S = Q K^T, dP = dO V^T, dS = P (dP - delta) * scale, dQ += bf16(dS) K.
+// dq_bf16 != nullptr: dQ is written once as bf16 (row stride ld_dq); else it is added into the fp32 dq_f32
+// [(q_shared ? 1 : nseq) * Sq][n_heads * 128] with red.global (with q_shared the images' contributions sum up).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                         const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                        const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dq,
-                        long long ld_dq, int Sq, int Skv, int n_heads, int kv_group, int causal, float scale) {
-  using Cfg = AttBwd2Cfg;
-  constexpr int D = Cfg::D, CH = Cfg::CH, STAGES = Cfg::STAGES;
+                        const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dq_bf16,
+                        long long ld_dq, float* __restrict__ dq_f32, int Sq, int Skv, int n_heads, int kv_group,
+                        int causal, int q_shared, float scale) {
+  using Cfg = AttBwdCfg;
+  constexpr int D = BWD_D;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* q_full = bars + 0;
-  uint64_t* ring_full = bars + 1;
-  uint64_t* ring_empty = bars + 1 + STAGES;
-  uint64_t* s_full = bars + 1 + 2 * STAGES;       // [3]
-  uint64_t* ds_full = s_full + 3;                 // [3]  (128 arrivals)
-  uint64_t* acc_done = ds_full + 3;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_done + 1);
+  uint64_t* q_full = bars;
+  uint64_t* c_full = bars + 1;
+  uint64_t* c_empty = bars + 1 + ATT_STAGES;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const int num_q_tiles = (Sq + 127) / 128;
-  const int q_tile = num_q_tiles - 1 - (int)blockIdx.x;            // heavy (late) tiles first
-  const int head = blockIdx.y, seq = blockIdx.z;
-  const int kv_head = head / kv_group;
+  const int q_tile = num_q_tiles - 1 - blockIdx.x;            // heavy (late) tiles first
   const int q0 = q_tile * 128;
-  const int kv_end = causal ? min(Skv, q0 + 128) : Skv;            // keys [0, kv_end) are visible to this tile
-  const int n_it = (kv_end + CH - 1) / CH;
+  const int head = blockIdx.y, seq = blockIdx.z;
+  const int q_seq = q_shared ? 0 : seq;
+  const int kv_head = head / kv_group;
+  const int n_all = (Skv + BWD_C - 1) / BWD_C;
+  const int n_c = causal ? min(n_all, (q0 + 128 + BWD_C - 1) / BWD_C) : n_all;
 
-  // The producer thread initialises the barriers its loads complete on and starts the resident Q / dO tiles and the
-  // first ring stages right away; TMEM allocation, the other barriers and the CTA-wide sync overlap the load latency
-  // (with ~10 chunks per CTA the prologue is a visible share of the kernel).
-  auto load_chunk = [&](int it) {
-    const int s = it % STAGES;
-    uint8_t* dst = smem + Cfg::OFF_RING + s * 2 * Cfg::CHUNK_BYTES;
-    mbar_arrive_expect_tx(&ring_full[s], 2 * Cfg::CHUNK_BYTES);
-    for (int a = 0; a < 2; ++a) {
-      tma_load_3d(dst + a * (CH * 128), &tmK, &ring_full[s], kv_head * D + a * 64, it * CH, seq);
-      tma_load_3d(dst + Cfg::CHUNK_BYTES + a * (CH * 128), &tmV, &ring_full[s], kv_head * D + a * 64, it * CH, seq);
-    }
-  };
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&ring_full[i], 1); mbar_init(&ring_empty[i], 1); }
+    for (int i = 0; i < ATT_STAGES; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 8); }
     fence_barrier_init();
-    mbar_arrive_expect_tx(q_full, 2 * Cfg::TILE_BYTES);
-    for (int a = 0; a < 2; ++a) {
-      tma_load_3d(smem + Cfg::OFF_RES0 + a * 16384, &tmQ, q_full, head * D + a * 64, q0, seq);
-      tma_load_3d(smem + Cfg::OFF_RES1 + a * 16384, &tmDO, q_full, head * D + a * 64, q0, seq);
-    }
-    for (int it = 0; it < n_it && it < STAGES; ++it) load_chunk(it);
   }
-  if (warp == 9) {
-    if (lane == 0) {
-      for (int i = 0; i < 3; ++i) { mbar_init(&s_full[i], 1); mbar_init(&ds_full[i], 128); }
-      mbar_init(acc_done, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // columns: dQ = 256..383; THREE S / dP buffers (b = chunk % 3): S[b] = b*64, dP[b] = 128 + b*64 for b < 2 and
-  // S[2] = 384, dP[2] = 448. With two buffers S(it+2) could only be issued after dS(it) had been consumed, so each compute
-  // group waited for "dQ MMA + next S/dP MMAs + commit latency" after every chunk (44 % of its time in the ncu sampling);
-  // with three, S/dP run two chunks ahead and never wait on the chunk being processed.
-  auto s_col = [&](int b) -> uint32_t { return b < 2 ? (uint32_t)(b * CH) : 384u; };
-  auto dp_col = [&](int b) -> uint32_t { return b < 2 ? (uint32_t)(128 + b * CH) : 448u; };
 
-  if (warp >= 8) {
-   setmaxnreg_dec<56>();
-   if (warp == 8) {
-    if (lane == 0) {
-      for (int it = STAGES; it < n_it; ++it) {       // the first STAGES chunks were issued before the CTA sync
-        mbar_wait(&ring_empty[it % STAGES], ((it / STAGES) - 1) & 1);
-        load_chunk(it);
+  if (wg == 2) {
+    if (threadIdx.x == 256) {
+      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
+      mbar_arrive_expect_tx(q_full, 2 * Cfg::TILE_BYTES);
+      for (int a = 0; a < 2; ++a) {
+        tma_load_3d(smem + a * Cfg::TILE_ATOM, &tmQ, q_full, head * D + a * 64, q0, q_seq);
+        tma_load_3d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmDO, q_full, head * D + a * 64, q0, seq);
+      }
+      for (int j = 0; j < n_c; ++j) {
+        const int s = j % ATT_STAGES;
+        if (j >= ATT_STAGES) mbar_wait(&c_empty[s], ((j / ATT_STAGES) - 1) & 1);
+        uint8_t* dst = smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES;
+        mbar_arrive_expect_tx(&c_full[s], 2 * Cfg::CHUNK_BYTES);
+        for (int a = 0; a < 2; ++a) {
+          tma_load_3d(dst + a * Cfg::CHUNK_ATOM, &tmK, &c_full[s], kv_head * D + a * 64, j * BWD_C, seq);
+          tma_load_3d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmV, &c_full[s], kv_head * D + a * 64, j * BWD_C,
+                      seq);
+        }
       }
     }
-   } else if (warp == 9) {
-    {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, CH, false, false);
-      constexpr uint32_t idesc_acc = make_idesc_bf16(128, D, false, true);
-      const bool leader = elect_one();
-      const uint64_t qd = desc_kmajor(smem_u32(smem + Cfg::OFF_RES0), 0), dod = desc_kmajor(smem_u32(smem + Cfg::OFF_RES1), 0);
-      auto issue_s = [&](int it) {
-        const int s = it % STAGES, b = it % 3;
-        mbar_wait(&ring_full[s], (it / STAGES) & 1);
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(smem + Cfg::OFF_RING + s * 2 * Cfg::CHUNK_BYTES);
-        const uint64_t kd = desc_kmajor(k_addr, 0), vd = desc_kmajor(k_addr + Cfg::CHUNK_BYTES, 0);
-        if (leader) {
-#pragma unroll
-          for (int k16 = 0; k16 < D / 16; ++k16) {    // S = Q K^T
-            const uint64_t oa = (uint64_t)((k16 >> 2) * (128 * 8) + (k16 & 3) * 2), ob = (uint64_t)((k16 >> 2) * (CH * 8) + (k16 & 3) * 2);
-            umma_ss(tmem_base + s_col(b), qd + oa, kd + ob, idesc_s, k16 > 0);
-          }
-#pragma unroll
-          for (int k16 = 0; k16 < D / 16; ++k16) {    // dP = dO V^T
-            const uint64_t oa = (uint64_t)((k16 >> 2) * (128 * 8) + (k16 & 3) * 2), ob = (uint64_t)((k16 >> 2) * (CH * 8) + (k16 & 3) * 2);
-            umma_ss(tmem_base + dp_col(b), dod + oa, vd + ob, idesc_s, k16 > 0);
-          }
-          umma_commit(&s_full[b]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      if (n_it > 1) issue_s(1);
-      for (int it = 0; it < n_it; ++it) {
-        // buffer (it+2) % 3 == (it-1) % 3 was released by the dQ MMA of chunk it-1, issued by this thread just before
-        if (it + 2 < n_it) issue_s(it + 2);
-        const int s = it % STAGES, b = it % 3;
-        mbar_wait(&ds_full[b], (it / 3) & 1);
-        tc_fence_after();
-        const uint64_t km = desc_mnmajor(smem_u32(smem + Cfg::OFF_RING + s * 2 * Cfg::CHUNK_BYTES), 0, CH);
-        if (leader) {
-#pragma unroll
-          for (int k16 = 0; k16 < CH / 16; ++k16)     // dQ += dS K   (A = dS in TMEM, B = K chunk read MN-major)
-            umma_ts(tmem_base + 256, tmem_base + dp_col(b) + k16 * 8, km + (uint64_t)(k16 * 128), idesc_acc,
-                    (it > 0 || k16 > 0));
-          umma_commit(&ring_empty[s]);
-        }
-        __syncwarp();
-      }
-      if (leader) umma_commit(acc_done);
-      __syncwarp();
-    }
-   }
   } else {
-    // ------------------------------ compute groups: thread = query row ------------------------------
-    setmaxnreg_inc<224>();
-    const int g = warp >> 2;
-    const int r = (warp & 3) * 32 + lane;
-    const int q_idx = q0 + r;
-    const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;
+    const FragPos fp = frag_pos();
+    const int qr[2] = {q0 + wg * 64 + fp.r0, q0 + wg * 64 + fp.r0 + 8};
     const float c = scale * LOG2E;
-    const long long sbase = ((long long)seq * n_heads + head) * Sq;
-    const float my_lse = q_idx < Sq ? lse[sbase + q_idx] * LOG2E : INFINITY;
-    const float my_delta = q_idx < Sq ? delta[sbase + q_idx] : 0.f;
-    for (int it = g; it < n_it; it += 2) {
-      const int kvc = it * CH;
-      const int b = it % 3;
-      const uint32_t tS = tmem_base + s_col(b) + lane_off, tDP = tmem_base + dp_col(b) + lane_off;
-      mbar_wait(&s_full[b], (it / 3) & 1);
-      tc_fence_after();
-      uint32_t sv[64], dpv[64];
-      tmem_ld_32x32b_x64(tS, sv);
-      tmem_ld_32x32b_x64(tDP, dpv);
-      tmem_wait_ld();
-      const bool need_mask = (kvc + CH > Skv) || (causal && kvc + CH > q0);     // uniform: last chunks only
-      if (need_mask) {
-        int last_visible = Skv - 1 - kvc;                                       // columns > this are masked
-        if (causal) last_visible = min(last_visible, q_idx - kvc);
+    const long long base = ((long long)seq * n_heads + head) * Sq;
+    float lse2[2], dl[2];
 #pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (i > last_visible) sv[i] = 0xff800000u;                            // -inf => p = 0
-      }
-#pragma unroll
-      for (int i = 0; i < 64; ++i) {
-        const float pv = fast_exp2(fmaf(__uint_as_float(sv[i]), c, -my_lse));
-        dpv[i] = __float_as_uint(pv * (__uint_as_float(dpv[i]) - my_delta) * scale);
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          pk[i] = pack_bf16(__uint_as_float(dpv[h * 32 + 2 * i]), __uint_as_float(dpv[h * 32 + 2 * i + 1]));
-        tmem_st_32x32b_x16(tDP + h * 16, pk);
-      }
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(&ds_full[b]);
+    for (int h = 0; h < 2; ++h) {
+      lse2[h] = qr[h] < Sq ? lse[base + qr[h]] * LOG2E : INFINITY;   // padded q: P = 0
+      dl[h] = qr[h] < Sq ? delta[base + qr[h]] : 0.f;
     }
-    // epilogue: group g stores dQ columns [g*64, g*64+64) of its row
-    mbar_wait(acc_done, 0);
-    tc_fence_after();
-    {
-      // every MMA is complete (acc_done): the K/V ring is free, 4 KB of it per warp stages the coalesced stores
-      const int row0 = q0 + (warp & 3) * 32;
-      uint8_t* stage = smem + Cfg::OFF_RING + warp * (32 * 128);
-      store_tile_rows<2>(tmem_base + 256 + g * 64 + lane_off, 1.f, stage, lane,
-                         dq + ((long long)seq * Sq + row0) * ld_dq + head * D + g * 64, ld_dq, Sq - row0);
+    float dqacc[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) dqacc[i] = 0.f;
+    const uint32_t q_addr = smem_u32(smem) + wg * 64 * 128;
+    const uint32_t do_addr = smem_u32(smem + Cfg::OFF_T1) + wg * 64 * 128;
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < n_c; ++j) {
+      const int s = j % ATT_STAGES;
+      const uint32_t k_addr = smem_u32(smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES);
+      const uint32_t v_addr = k_addr + Cfg::CHUNK_BYTES;
+      mbar_wait(&c_full[s], (j / ATT_STAGES) & 1);
+      float sv[32], dp[32];
+      wgmma_fence();
+      mma_qk_64<D>(sv, q_addr, Cfg::TILE_ATOM, k_addr, Cfg::CHUNK_ATOM);
+      mma_qk_64<D>(dp, do_addr, Cfg::TILE_ATOM, v_addr, Cfg::CHUNK_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(sv);
+      reg_fence(dp);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int kv = j * BWD_C + 8 * i + fp.c0 + (e & 1);
+          const int h = e >> 1;
+          const bool masked = kv >= Skv || (causal && kv > qr[h]);
+          const float p = masked ? 0.f : fast_exp2(sv[4 * i + e] * c - lse2[h]);
+          dp[4 * i + e] = p * (dp[4 * i + e] - dl[h]) * scale;
+        }
+      uint32_t da[4][4];
+      acc_to_afrag<4>(dp, da);
+      reg_fence(dqacc);
+      wgmma_fence();
+      mma_pv<D, 4>(dqacc, da, k_addr, Cfg::CHUNK_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(dqacc);
+      if (lane == 0) mbar_arrive(&c_empty[s]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int q = qr[h];
+      if (q >= Sq) continue;
+      if (dq_bf16) {
+        bf16* row = dq_bf16 + ((long long)seq * Sq + q) * ld_dq + head * D + fp.c0;
+#pragma unroll
+        for (int i = 0; i < D / 8; ++i)
+          *reinterpret_cast<uint32_t*>(row + 8 * i) = pack_bf16(dqacc[4 * i + 2 * h], dqacc[4 * i + 2 * h + 1]);
+      } else {
+        float* row = dq_f32 + ((long long)q_seq * Sq + q) * ((long long)n_heads * D) + head * D + fp.c0;
+#pragma unroll
+        for (int i = 0; i < D / 8; ++i)
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(row + 8 * i), "f"(dqacc[4 * i + 2 * h]),
+                       "f"(dqacc[4 * i + 2 * h + 1])
+                       : "memory");
+      }
+    }
   }
 }
 
@@ -1367,13 +594,6 @@ static int make_qkv_tmap_rows(CUtensorMap* tm, const void* ptr, long long ld, in
   uint64_t dims[3] = {(uint64_t)cols, (uint64_t)S, (uint64_t)nseq};
   uint64_t str[2] = {(uint64_t)ld * 2, (uint64_t)S * ld * 2};
   uint32_t box[3] = {64, (uint32_t)box_rows, 1};
-  return make_tmap_bf16(tm, ptr, 3, dims, str, box);
-}
-
-static int make_qkv_tmap(CUtensorMap* tm, const void* ptr, long long ld, int nseq, int S, int cols) {
-  uint64_t dims[3] = {(uint64_t)cols, (uint64_t)S, (uint64_t)nseq};
-  uint64_t str[2] = {(uint64_t)ld * 2, (uint64_t)S * ld * 2};
-  uint32_t box[3] = {64, 128, 1};
   return make_tmap_bf16(tm, ptr, 3, dims, str, box);
 }
 
@@ -1385,21 +605,8 @@ static int launch_att_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CU
   auto kern = attention_fwd_kernel<D, CAUSAL>;
   B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)Cfg::SMEM_BYTES));
   dim3 grid((Sq + ATT_BQ - 1) / ATT_BQ, n_heads, nseq);
-  kern<<<grid, 160, Cfg::SMEM_BYTES, st>>>(tq, tk, tv, out, ld_out, lse, Sq, Skv, n_heads, kv_group, q_shared, scale);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int D, bool CAUSAL>
-static int launch_att_fwd2(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, bf16* out,
-                           long long ld_out, float* lse, int nseq, int Sq, int Skv, int n_heads, int kv_group,
-                           int q_shared, float scale, cudaStream_t st) {
-  using Cfg = AttFwd2Cfg<D>;
-  auto kern = attention_fwd2_kernel<D, CAUSAL>;
-  B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)Cfg::SMEM_BYTES));
-  const int num_q_tiles = (Sq + ATT_BQ - 1) / ATT_BQ;
-  dim3 grid((num_q_tiles + 1) / 2, n_heads, nseq);
-  kern<<<grid, 384, Cfg::SMEM_BYTES, st>>>(tq, tk, tv, out, ld_out, lse, Sq, Skv, n_heads, kv_group, q_shared, scale);
+  kern<<<grid, ATT_THREADS, Cfg::SMEM_BYTES, st>>>(tq, tk, tv, out, ld_out, lse, Sq, Skv, n_heads, kv_group, q_shared,
+                                                   scale);
   B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1407,13 +614,6 @@ static int launch_att_fwd2(const CUtensorMap& tq, const CUtensorMap& tk, const C
 }  // namespace b200
 
 using namespace b200;
-
-// 0: single-tile kernel (round 1), 1 (default): two-tile ping-pong kernel with P in TMEM
-static int g_att_fwd_variant = 1;
-extern "C" int rlaifv_attention_set_variant(int fwd_variant) {
-  g_att_fwd_variant = fwd_variant;
-  return 0;
-}
 
 static int attention_fwd_impl(const void* q, long long ld_q, const void* k, const void* v, long long ld_kv, void* out,
                               long long ld_out, float* lse, int nseq, int Sq, int Skv, int n_heads, int n_kv_heads,
@@ -1426,23 +626,15 @@ static int attention_fwd_impl(const void* q, long long ld_q, const void* k, cons
   B200_REQUIRE(nseq > 0 && Sq > 0 && Skv > 0, "attention_fwd: empty problem");
   CUtensorMap tq, tk, tv;
   int rc;
-  if ((rc = make_qkv_tmap(&tq, q, ld_q, q_shared ? 1 : nseq, Sq, n_heads * head_dim))) return rc;
-  if ((rc = make_qkv_tmap(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim))) return rc;
-  if ((rc = make_qkv_tmap(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, q_shared ? 1 : nseq, Sq, n_heads * head_dim, ATT_BQ))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, ATT_BKV))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, ATT_BKV))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int g = n_heads / n_kv_heads;
   bf16* o = (bf16*)out;
-  if (g_att_fwd_variant == 1) {
-    if (head_dim == 128)
-      return causal ? launch_att_fwd2<128, true>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st)
-                    : launch_att_fwd2<128, false>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st);
-    return causal ? launch_att_fwd2<64, true>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st)
-                  : launch_att_fwd2<64, false>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st);
-  }
-  if (head_dim == 128) {
+  if (head_dim == 128)
     return causal ? launch_att_fwd<128, true>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st)
                   : launch_att_fwd<128, false>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st);
-  }
   return causal ? launch_att_fwd<64, true>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st)
                 : launch_att_fwd<64, false>(tq, tk, tv, o, ld_out, lse, nseq, Sq, Skv, n_heads, g, q_shared, scale, st);
 }
@@ -1470,53 +662,21 @@ extern "C" int rlaifv_cross_attention_fwd(const void* q, long long ld_q, const v
                             q_shared, scale, stream);
 }
 
+// delta, then the dK/dV kernel, then the dQ kernel. dq != nullptr: dQ written as bf16 [nseq*Sq rows][ld_dq];
+// else added into dq_f32 (fp32 [(q_shared ? 1 : nseq) * Sq][n_heads*128], zeroed by the caller).
 static int attention_bwd_impl(const void* q, long long ld_q, const void* k, const void* v, long long ld_kv,
                               const void* out, long long ld_out, const void* d_out, long long ld_dout, const float* lse,
-                              float* dq_f32, void* dk, void* dv, long long ld_dkv, float* delta_ws, int nseq, int Sq,
-                              int Skv, int n_heads, int n_kv_heads, int head_dim, int causal, int q_shared, float scale,
-                              void* stream) {
+                              void* dq, long long ld_dq, float* dq_f32, void* dk, void* dv, long long ld_dkv,
+                              float* delta_ws, int nseq, int Sq, int Skv, int n_heads, int n_kv_heads, int head_dim,
+                              int causal, int q_shared, float scale, void* stream) {
   B200_REQUIRE(head_dim == 128, "attention_bwd: head_dim must be 128 (got %d)", head_dim);
   B200_REQUIRE(n_kv_heads > 0 && n_heads % n_kv_heads == 0, "attention_bwd: bad head counts %d / %d", n_heads,
                n_kv_heads);
   B200_REQUIRE(!causal || Sq == Skv, "attention_bwd: causal needs Sq == Skv (%d vs %d)", Sq, Skv);
   B200_REQUIRE(nseq > 0 && Sq > 0 && Skv > 0, "attention_bwd: empty problem");
-  cudaStream_t st = (cudaStream_t)stream;
-  {
-    const long long total = (long long)nseq * Sq * n_heads;
-    long long blocks = (total + 7) / 8;
-    if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
-    attention_delta_kernel<<<(int)blocks, 256, 0, st>>>((const bf16*)out, ld_out, (const bf16*)d_out, ld_dout,
-                                                        delta_ws, nseq, Sq, n_heads, head_dim);
-    B200_CHECK_CUDA(cudaGetLastError());
-  }
-  CUtensorMap tq, tk, tv, tdo;
-  int rc;
-  if ((rc = make_qkv_tmap(&tq, q, ld_q, q_shared ? 1 : nseq, Sq, n_heads * head_dim))) return rc;
-  if ((rc = make_qkv_tmap(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim))) return rc;
-  if ((rc = make_qkv_tmap(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim))) return rc;
-  if ((rc = make_qkv_tmap(&tdo, d_out, ld_dout, nseq, Sq, n_heads * head_dim))) return rc;
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_kernel, (int)AttBwdCfg::SMEM_BYTES));
-  dim3 grid((Skv + 127) / 128, n_kv_heads, nseq);
-  attention_bwd_kernel<<<grid, 160, AttBwdCfg::SMEM_BYTES, st>>>(tq, tk, tv, tdo, lse, delta_ws, dq_f32, (bf16*)dk,
-                                                                 (bf16*)dv, ld_dkv, Sq, Skv, n_heads,
-                                                                 n_heads / n_kv_heads, causal, q_shared, scale);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// Split backward for self-attention (causal or not, Sq == Skv or not; per-sequence queries): dq is written as bf16
-// [nseq*Sq rows][ld_dq] (it may be the q column block of a fused dqkv buffer), dk/dv as before; no zero-fill needed.
-extern "C" int rlaifv_attention_bwd_split(const void* q, long long ld_q, const void* k, const void* v, long long ld_kv,
-                                          const void* out, long long ld_out, const void* d_out, long long ld_dout,
-                                          const float* lse, void* dq, long long ld_dq, void* dk, void* dv,
-                                          long long ld_dkv, float* delta_ws, int nseq, int Sq, int Skv, int n_heads,
-                                          int n_kv_heads, int head_dim, int causal, float scale, void* stream) {
-  B200_REQUIRE(head_dim == 128, "attention_bwd_split: head_dim must be 128 (got %d)", head_dim);
-  B200_REQUIRE(n_kv_heads > 0 && n_heads % n_kv_heads == 0, "attention_bwd_split: bad head counts %d / %d", n_heads,
-               n_kv_heads);
-  B200_REQUIRE(!causal || Sq == Skv, "attention_bwd_split: causal needs Sq == Skv (%d vs %d)", Sq, Skv);
-  B200_REQUIRE(nseq > 0 && Sq > 0 && Skv > 0, "attention_bwd_split: empty problem");
-  B200_REQUIRE(ld_dq % 8 == 0 && ld_dkv % 8 == 0 && ((uintptr_t)dq & 15) == 0, "attention_bwd_split: dq alignment");
+  B200_REQUIRE(ld_q % 8 == 0 && ld_kv % 8 == 0 && ld_dout % 8 == 0, "attention_bwd: ld must be a multiple of 8");
+  B200_REQUIRE(dq ? (ld_dq % 2 == 0 && ((uintptr_t)dq & 3) == 0) : dq_f32 != nullptr, "attention_bwd: dq alignment");
+  B200_REQUIRE(ld_dkv % 2 == 0, "attention_bwd: ld_dkv must be even");
   cudaStream_t st = (cudaStream_t)stream;
   {
     const long long total = (long long)nseq * Sq * n_heads;
@@ -1527,34 +687,46 @@ extern "C" int rlaifv_attention_bwd_split(const void* q, long long ld_q, const v
     B200_CHECK_CUDA(cudaGetLastError());
   }
   const int g = n_heads / n_kv_heads;
+  const int q_nseq = q_shared ? 1 : nseq;
   int rc;
   CUtensorMap tq, tk, tv, tdo;
   // dK / dV: K, V resident (128-row boxes), Q / dO streamed in 64-row chunks
-  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, nseq, Sq, n_heads * head_dim, 64))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tdo, d_out, ld_dout, nseq, Sq, n_heads * head_dim, 64))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, q_nseq, Sq, n_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tdo, d_out, ld_dout, nseq, Sq, n_heads * head_dim, BWD_C))) return rc;
   if ((rc = make_qkv_tmap_rows(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, 128))) return rc;
   if ((rc = make_qkv_tmap_rows(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, 128))) return rc;
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dkv_kernel, (int)AttBwd2Cfg::SMEM_BYTES));
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dq_kernel, (int)AttBwd2Cfg::SMEM_BYTES));
+  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dkv_kernel, (int)AttBwdCfg::SMEM_BYTES));
+  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dq_kernel, (int)AttBwdCfg::SMEM_BYTES));
   {
     dim3 grid((Skv + 127) / 128, n_kv_heads, nseq);
-    attention_bwd_dkv_kernel<<<grid, 384, AttBwd2Cfg::SMEM_BYTES, st>>>(tq, tk, tv, tdo, lse, delta_ws, (bf16*)dk,
-                                                                        (bf16*)dv, ld_dkv, Sq, Skv, n_heads, g, causal,
-                                                                        scale);
+    attention_bwd_dkv_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
+        tq, tk, tv, tdo, lse, delta_ws, (bf16*)dk, (bf16*)dv, ld_dkv, Sq, Skv, n_heads, g, causal, q_shared, scale);
     B200_CHECK_CUDA(cudaGetLastError());
   }
   // dQ: Q, dO resident, K / V streamed in 64-row chunks
-  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, nseq, Sq, n_heads * head_dim, 128))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, q_nseq, Sq, n_heads * head_dim, 128))) return rc;
   if ((rc = make_qkv_tmap_rows(&tdo, d_out, ld_dout, nseq, Sq, n_heads * head_dim, 128))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, 64))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, 64))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, BWD_C))) return rc;
   {
     dim3 grid((Sq + 127) / 128, n_heads, nseq);
-    attention_bwd_dq_kernel<<<grid, 384, AttBwd2Cfg::SMEM_BYTES, st>>>(tq, tk, tv, tdo, lse, delta_ws, (bf16*)dq, ld_dq,
-                                                                       Sq, Skv, n_heads, g, causal, scale);
+    attention_bwd_dq_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
+        tq, tk, tv, tdo, lse, delta_ws, (bf16*)dq, ld_dq, dq_f32, Sq, Skv, n_heads, g, causal, q_shared, scale);
     B200_CHECK_CUDA(cudaGetLastError());
   }
   return 0;
+}
+
+// Split backward for self-attention (causal or not, Sq == Skv or not; per-sequence queries): dq is written as bf16
+// [nseq*Sq rows][ld_dq] (it may be the q column block of a fused dqkv buffer), dk/dv as before; no zero-fill needed.
+extern "C" int rlaifv_attention_bwd_split(const void* q, long long ld_q, const void* k, const void* v, long long ld_kv,
+                                          const void* out, long long ld_out, const void* d_out, long long ld_dout,
+                                          const float* lse, void* dq, long long ld_dq, void* dk, void* dv,
+                                          long long ld_dkv, float* delta_ws, int nseq, int Sq, int Skv, int n_heads,
+                                          int n_kv_heads, int head_dim, int causal, float scale, void* stream) {
+  B200_REQUIRE(dq != nullptr, "attention_bwd_split: dq missing");
+  return attention_bwd_impl(q, ld_q, k, v, ld_kv, out, ld_out, d_out, ld_dout, lse, dq, ld_dq, nullptr, dk, dv, ld_dkv,
+                            delta_ws, nseq, Sq, Skv, n_heads, n_kv_heads, head_dim, causal, 0, scale, stream);
 }
 
 // dq_f32 [nseq*S][n_heads*128] must be zeroed by the caller; delta_ws fp32 [nseq*n_heads*S].
@@ -1563,16 +735,16 @@ extern "C" int rlaifv_attention_bwd(const void* q, const void* k, const void* v,
                                     const float* lse, float* dq_f32, void* dk, void* dv, long long ld_dkv,
                                     float* delta_ws, int nseq, int S, int n_heads, int head_dim, float scale,
                                     void* stream) {
-  return attention_bwd_impl(q, ld_qkv, k, v, ld_qkv, out, ld_out, d_out, ld_dout, lse, dq_f32, dk, dv, ld_dkv, delta_ws,
+  return attention_bwd_impl(q, ld_qkv, k, v, ld_qkv, out, ld_out, d_out, ld_dout, lse, nullptr, 0, dq_f32, dk, dv, ld_dkv, delta_ws,
                             nseq, S, S, n_heads, n_heads, head_dim, 1, 0, scale, stream);
 }
-// GQA: dk/dv hold n_kv_heads heads (sum over the query heads of each group is formed in TMEM).
+// GQA: dk/dv hold n_kv_heads heads (sum over the query heads of each group is formed in registers).
 extern "C" int rlaifv_attention_bwd_gqa(const void* q, const void* k, const void* v, long long ld_qkv,
                                         const void* out, long long ld_out, const void* d_out, long long ld_dout,
                                         const float* lse, float* dq_f32, void* dk, void* dv, long long ld_dkv,
                                         float* delta_ws, int nseq, int S, int n_heads, int n_kv_heads, int head_dim,
                                         float scale, void* stream) {
-  return attention_bwd_impl(q, ld_qkv, k, v, ld_qkv, out, ld_out, d_out, ld_dout, lse, dq_f32, dk, dv, ld_dkv, delta_ws,
+  return attention_bwd_impl(q, ld_qkv, k, v, ld_qkv, out, ld_out, d_out, ld_dout, lse, nullptr, 0, dq_f32, dk, dv, ld_dkv, delta_ws,
                             nseq, S, S, n_heads, n_kv_heads, head_dim, 1, 0, scale, stream);
 }
 // Cross-attention backward (non-causal, head_dim 128). dq_f32 fp32 [(q_shared ? 1 : nseq) * Sq][n_heads*128],
@@ -1583,6 +755,6 @@ extern "C" int rlaifv_cross_attention_bwd(const void* q, long long ld_q, const v
                                           const float* lse, float* dq_f32, void* dk, void* dv, long long ld_dkv,
                                           float* delta_ws, int nseq, int Sq, int Skv, int n_heads, int head_dim,
                                           int q_shared, float scale, void* stream) {
-  return attention_bwd_impl(q, ld_q, k, v, ld_kv, out, ld_out, d_out, ld_dout, lse, dq_f32, dk, dv, ld_dkv, delta_ws,
+  return attention_bwd_impl(q, ld_q, k, v, ld_kv, out, ld_out, d_out, ld_dout, lse, nullptr, 0, dq_f32, dk, dv, ld_dkv, delta_ws,
                             nseq, Sq, Skv, n_heads, n_heads, head_dim, 0, q_shared, scale, stream);
 }

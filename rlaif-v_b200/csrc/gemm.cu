@@ -1,6 +1,7 @@
-// bf16 x bf16 -> fp32(TMEM) -> bf16 GEMM for sm_100a: TMA-staged SWIZZLE_128B shared-memory tiles
-// feeding tcgen05.mma (UMMA 128 x BN x 16), persistent warp-specialised CTAs, double-buffered
-// TMEM accumulators so the epilogue of tile i overlaps the main loop of tile i+1.
+// bf16 x bf16 -> fp32 -> bf16 GEMM for sm_90a: TMA-staged SWIZZLE_128B shared-memory tiles feeding wgmma.mma_async
+// (64 x BN x 16 per warpgroup), persistent warp-specialised CTAs: one producer warpgroup issues the TMA loads of a
+// multi-stage ring, two math warpgroups each own 64 rows of the 128 x BN tile and run the epilogue straight from their
+// accumulator registers while the producer already streams the next tile's operands.
 //
 // One kernel covers the three operand forms a linear layer needs (reference call sites: every
 // nn.Linear inside HF LlamaDecoderLayer / CLIPEncoderLayer / mm_projector —
@@ -9,10 +10,10 @@
 //   dgrad    dX[M,K] = dY[M,N] * W[N,K]        A K-major,  B MN-major
 //   wgrad    dW[N,K] = dY[M,N]^T * X[M,K]      A MN-major, B MN-major
 // "K-major" = contraction index contiguous in memory; "MN-major" = the tensor is stored
-// [contraction][M or N] row-major. No transposes are ever materialised.
+// [contraction][M or N] row-major. No transposes are ever materialised: wgmma reads MN-major tiles transposed.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc),
-// warps 2..5 = epilogue (TMEM lane quadrant = warp % 4).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues), warpgroups 1, 2 = MMA + epilogue of rows
+// [0, 64) and [64, 128) of the tile.
 #include "common.cuh"
 #include "host_util.h"
 
@@ -27,17 +28,15 @@ struct GemmEpilogue {
   int act;         // 0 none, 1 GELU(erf), 2 quick_gelu (x*sigmoid(1.702x))
   int accumulate;  // C = C + result (fp32 add of the old bf16 value)
   int group_m;     // raster: tiles are walked m-fastest inside groups of `group_m` row-blocks
-  int debug;       // profiling only: bit0 skip global stores, bit1 skip the TMEM loads as well
-  int dynamic;     // 1: tiles drawn from the global counter; 0: static round-robin (tile = cta + i*grid)
+  int debug;       // profiling only: bit0 skip global stores
   float alpha;     // != 1: result = bf16(bf16(acc) * alpha) first (LoRA scaling, peft: lora_B(...) * scaling)
-  int tma_store;   // 1: C leaves through swizzled shared memory + cp.async.bulk.tensor stores (full 128-byte rows)
   const bf16* glu; // non-null: fused SwiGLU backward. The accumulator tile is d(act) [M, N = F]; glu = [gate | up] rows
   long long ld_glu;//   [M, 2F]; C = d[gate | up] [M, 2F]: C[:, n] = d*u*silu'(g), C[:, F + n] = d*silu(g)  (d = bf16(acc))
-  int l2;          // L2 policy of the CTA-pair kernel: bits 0-1 A loads, 2-3 B loads, 4-5 C stores (0 normal, 1 evict
-                   // first, 2 evict last); bit 6: raster groups column blocks (n-fastest inside groups of group_m)
+  int l2;          // L2 policy of the operand loads: bits 0-1 A, 2-3 B (0 normal, 1 evict first, 2 evict last);
+                   // bit 6: raster groups column blocks (n-fastest inside groups of group_m)
 };
 
-// Optional second operand pair accumulated into the same TMEM tile after the first K loop:
+// Optional second operand pair accumulated into the same accumulator tile after the first K loop:
 //   C = A1 * B1^T + A2[:, koff : koff + K2] * B2^T,   koff = (n0 / n_sub) * r   (0 when n_sub == 0).
 // This is how the LoRA rank-r update rides in the same CTA pass as the frozen base GEMM
 // (forward: A2 = s*A(x) [M, g*r], B2 = stacked lora_B [N, r]; dgrad: A2 = s*dy*B [M, g*r], B2 = stacked lora_A).
@@ -49,33 +48,16 @@ struct GemmSecondSource {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_THREADS = 192;
-// Epilogue staging for the TMA store of C: each of the 4 epilogue warps owns two [32 rows x 64 bf16] SWIZZLE_128B
-// buffers (4 KB each, double-buffered against the asynchronous store) = 32 KB per CTA.
-constexpr uint32_t EPI_BUF_BYTES = 32 * 128;
-constexpr uint32_t EPI_STAGE_BYTES = 4 * 2 * EPI_BUF_BYTES;
-
-// Dynamic tile scheduler: CTAs pull tile indices from a global counter, so a CTA that becomes
-// resident late (an NCCL kernel of the overlapped ZeRO-2 reduce-scatter is holding its SM) simply
-// processes fewer tiles instead of stretching the whole GEMM. The last CTA to leave resets the
-// counter pair, so no memset is needed between launches; a pool of 64 pairs is cycled per launch.
-struct TileCounter {
-  unsigned int next;
-  unsigned int done;
-};
-__device__ TileCounter g_tile_counters[64];
-constexpr int GEMM_TQ = 4;   // depth of the in-CTA tile-index queue (producer -> MMA / epilogue warps)
-static TileCounter* g_counter_pool = nullptr;
-static unsigned int g_launch_seq = 0;
+constexpr int GEMM_THREADS = 384;
+constexpr uint32_t ATOM_BYTES = 64 * 128;   // one [64 rows][64 bf16] SWIZZLE_128B atom
 
 template <int BN>
 struct GemmCfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : 6;
+  static constexpr int STAGES = (BN == 256) ? 4 : 6;    // 192 KB of the 227 KB a block may use
   static constexpr uint32_t A_BYTES = GEMM_BM * GEMM_BK * 2;
   static constexpr uint32_t B_BYTES = BN * GEMM_BK * 2;
   static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr uint32_t TMEM_COLS = 2 * BN;
-  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + EPI_STAGE_BYTES + 512 + 1024;  // + barriers/queue + align
+  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;  // + barriers + alignment
 };
 
 __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int GROUP_M, int& m_blk, int& n_blk,
@@ -99,309 +81,127 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   return v;
 }
 
-
-// Epilogue math for 32 consecutive accumulator columns of one output row (registers r[32]).
-__device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], int col0, int N, bf16* c_row,
-                                               const bf16* r_row, const GemmEpilogue& epi) {
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const int col = col0 + g * 8;
-    if (col < N) {
-      float v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(r[g * 8 + j]);
-      if (epi.alpha != 1.0f) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = bf16_round(bf16_round(v[j]) * epi.alpha);
-      }
-      if (epi.bias) {
-        uint4 b4 = __ldg(reinterpret_cast<const uint4*>(epi.bias + col));
-        float2 b0 = unpack_bf16(b4.x), b1 = unpack_bf16(b4.y), b2 = unpack_bf16(b4.z), b3 = unpack_bf16(b4.w);
-        v[0] += b0.x; v[1] += b0.y; v[2] += b1.x; v[3] += b1.y;
-        v[4] += b2.x; v[5] += b2.y; v[6] += b3.x; v[7] += b3.y;
-      }
-      if (epi.act) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = apply_act(bf16_round(v[j]), epi.act);
-      }
-      if (r_row) {
-        uint4 q4 = *reinterpret_cast<const uint4*>(r_row + col);
-        float2 q0 = unpack_bf16(q4.x), q1 = unpack_bf16(q4.y), q2 = unpack_bf16(q4.z), q3 = unpack_bf16(q4.w);
-        // reference adds two bf16 tensors: round the linear output first
-        v[0] = bf16_round(v[0]) + q0.x; v[1] = bf16_round(v[1]) + q0.y;
-        v[2] = bf16_round(v[2]) + q1.x; v[3] = bf16_round(v[3]) + q1.y;
-        v[4] = bf16_round(v[4]) + q2.x; v[5] = bf16_round(v[5]) + q2.y;
-        v[6] = bf16_round(v[6]) + q3.x; v[7] = bf16_round(v[7]) + q3.y;
-      }
-      if (epi.accumulate) {
-        uint4 o4 = *reinterpret_cast<const uint4*>(c_row + col);
-        float2 o0 = unpack_bf16(o4.x), o1 = unpack_bf16(o4.y), o2 = unpack_bf16(o4.z), o3 = unpack_bf16(o4.w);
-        v[0] += o0.x; v[1] += o0.y; v[2] += o1.x; v[3] += o1.y;
-        v[4] += o2.x; v[5] += o2.y; v[6] += o3.x; v[7] += o3.y;
-      }
-      uint4 o;
-      o.x = pack_bf16(v[0], v[1]);
-      o.y = pack_bf16(v[2], v[3]);
-      o.z = pack_bf16(v[4], v[5]);
-      o.w = pack_bf16(v[6], v[7]);
-      *reinterpret_cast<uint4*>(c_row + col) = o;
-    }
+// Epilogue of two adjacent accumulator columns (col, col + 1) of one output row.
+__device__ __forceinline__ void epilogue_pair(float v0, float v1, long long row, int col, const GemmEpilogue& epi) {
+  if (epi.alpha != 1.0f) {
+    v0 = bf16_round(bf16_round(v0) * epi.alpha);
+    v1 = bf16_round(bf16_round(v1) * epi.alpha);
   }
-}
-
-// Same math as epilogue_chunk, but the 32 columns go to this lane's row of the warp's swizzled staging buffer
-// (`half` = which 64-byte half of the 128-byte row) instead of straight to global memory.
-__device__ __forceinline__ void epilogue_chunk_staged(const uint32_t (&r)[32], int col0, int N, const bf16* c_row,
-                                                      const bf16* r_row, const GemmEpilogue& epi, bool accumulate,
-                                                      uint8_t* stage_row, int half, int lane) {
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const int col = col0 + g * 8;
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(r[g * 8 + j]);
-    if (col < N) {
-      if (epi.alpha != 1.0f) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = bf16_round(bf16_round(v[j]) * epi.alpha);
-      }
-      if (epi.bias) {
-        uint4 b4 = __ldg(reinterpret_cast<const uint4*>(epi.bias + col));
-        float2 b0 = unpack_bf16(b4.x), b1 = unpack_bf16(b4.y), b2 = unpack_bf16(b4.z), b3 = unpack_bf16(b4.w);
-        v[0] += b0.x; v[1] += b0.y; v[2] += b1.x; v[3] += b1.y;
-        v[4] += b2.x; v[5] += b2.y; v[6] += b3.x; v[7] += b3.y;
-      }
-      if (epi.act) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = apply_act(bf16_round(v[j]), epi.act);
-      }
-      if (r_row) {
-        uint4 q4 = *reinterpret_cast<const uint4*>(r_row + col);
-        float2 q0 = unpack_bf16(q4.x), q1 = unpack_bf16(q4.y), q2 = unpack_bf16(q4.z), q3 = unpack_bf16(q4.w);
-        v[0] = bf16_round(v[0]) + q0.x; v[1] = bf16_round(v[1]) + q0.y;
-        v[2] = bf16_round(v[2]) + q1.x; v[3] = bf16_round(v[3]) + q1.y;
-        v[4] = bf16_round(v[4]) + q2.x; v[5] = bf16_round(v[5]) + q2.y;
-        v[6] = bf16_round(v[6]) + q3.x; v[7] = bf16_round(v[7]) + q3.y;
-      }
-      if (accumulate) {
-        uint4 o4 = *reinterpret_cast<const uint4*>(c_row + col);
-        float2 o0 = unpack_bf16(o4.x), o1 = unpack_bf16(o4.y), o2 = unpack_bf16(o4.z), o3 = unpack_bf16(o4.w);
-        v[0] += o0.x; v[1] += o0.y; v[2] += o1.x; v[3] += o1.y;
-        v[4] += o2.x; v[5] += o2.y; v[6] += o3.x; v[7] += o3.y;
-      }
-    }
-    uint4 o;
-    o.x = pack_bf16(v[0], v[1]);
-    o.y = pack_bf16(v[2], v[3]);
-    o.z = pack_bf16(v[4], v[5]);
-    o.w = pack_bf16(v[6], v[7]);
-    const int chunk = (half * 4 + g) ^ (lane & 7);              // SWIZZLE_128B: 16-byte chunk index XOR (row % 8)
-    *reinterpret_cast<uint4*>(stage_row + chunk * 16) = o;
+  if (epi.bias) {
+    const float2 b = unpack_bf16(__ldg(reinterpret_cast<const unsigned int*>(epi.bias + col)));
+    v0 += b.x;
+    v1 += b.y;
   }
-}
-
-// Epilogue of one tile for one warp (32 rows): TMEM -> registers -> (math) -> swizzled smem -> TMA store, 64 columns at
-// a time, double-buffered against the asynchronous store. row0 = first row of this warp's 32-row slab.
-template <int BN>
-__device__ __forceinline__ void epilogue_tile_tma(uint32_t t_addr, long long row0, long long row, bool row_ok, int n0,
-                                                  int N, const GemmEpilogue& epi, const CUtensorMap* tmC,
-                                                  uint8_t* warp_stage, int lane, int& buf_sel) {
-  bf16* c_row = epi.C + row * epi.ldc;
-  const bf16* r_row = epi.residual ? epi.residual + row * epi.ldr : nullptr;
-#pragma unroll 1
-  for (int c64 = 0; c64 < BN / 64; ++c64) {
-    const int col0 = n0 + c64 * 64;
-    if (col0 >= N) break;
-    uint8_t* buf = warp_stage + buf_sel * EPI_BUF_BYTES;
-    if (lane == 0) tma_store_wait_read<1>();     // the store that last read `buf` (two issues ago) is done with it
-    __syncwarp();
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(t_addr + c64 * 64 + half * 32, r);
-      tmem_wait_ld();
-      // rows beyond M come from zero-filled OOB operand rows and are clipped by the tensor map on the way out; they
-      // must not touch the residual / C rows (addresses past the tensor)
-      epilogue_chunk_staged(r, col0 + half * 32, N, c_row, row_ok ? r_row : nullptr, epi,
-                            row_ok && epi.accumulate != 0, buf + lane * 128, half, lane);
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      if (epi.l2 & 0x30) tma_store_2d_hint(tmC, buf, col0, (int)row0, l2_policy((epi.l2 >> 4) & 3));
-      else tma_store_2d(tmC, buf, col0, (int)row0);
-      tma_store_commit();
-    }
-    buf_sel ^= 1;
+  if (epi.act) {
+    v0 = apply_act(bf16_round(v0), epi.act);
+    v1 = apply_act(bf16_round(v1), epi.act);
   }
+  if (epi.residual) {
+    // reference adds two bf16 tensors: round the linear output first
+    const float2 q = unpack_bf16(*reinterpret_cast<const uint32_t*>(epi.residual + row * epi.ldr + col));
+    v0 = bf16_round(v0) + q.x;
+    v1 = bf16_round(v1) + q.y;
+  }
+  uint32_t* c = reinterpret_cast<uint32_t*>(epi.C + row * epi.ldc + col);
+  if (epi.accumulate) {
+    const float2 o = unpack_bf16(*c);
+    v0 += o.x;
+    v1 += o.y;
+  }
+  *c = pack_bf16(v0, v1);
 }
 
 // Fused SwiGLU backward (HF llama/modeling_llama.py:182-184 under autograd): the GEMM computes d(act) = dy @ W_down for
-// a 256-column slice of F; instead of writing it out for a separate elementwise pass (0.4 GB written + read back per
-// layer, one more launch) the epilogue reads the matching gate / up values and writes d(gate) and d(up) straight into
-// the [M, 2F] gradient of the fused gate|up projection. d is rounded to bf16 first (the reference materialises it), the
-// arithmetic is swiglu_bwd_kernel's (rowops.cu). Uses both staging buffers of the warp per 64-column step (one for each
-// output half), so it waits for the previous step's two stores before restaging.
-template <int BN>
-__device__ __forceinline__ void epilogue_tile_glu(uint32_t t_addr, long long row0, long long row, bool row_ok, int n0,
-                                                  int N, const GemmEpilogue& epi, const CUtensorMap* tmC,
-                                                  uint8_t* warp_stage, int lane) {
+// a slice of F; instead of writing it out for a separate elementwise pass (one more launch, d(act) written and read
+// back) the epilogue reads the matching gate / up values and writes d(gate) and d(up) straight into the [M, 2F]
+// gradient of the fused gate|up projection. d is rounded to bf16 first (the reference materialises it); the arithmetic
+// is swiglu_bwd_kernel's (rowops.cu) with an approximate reciprocal (2 ulp, far below the bf16 rounding of the result).
+__device__ __forceinline__ void epilogue_pair_glu(float v0, float v1, long long row, int col, int N,
+                                                  const GemmEpilogue& epi) {
   const bf16* g_row = epi.glu + row * epi.ld_glu;
-  uint8_t* buf_g = warp_stage;
-  uint8_t* buf_u = warp_stage + EPI_BUF_BYTES;
-  // gate / up values of one 64-column step: 8 + 8 16-byte loads per lane (this lane's row), fetched one step ahead of
-  // the arithmetic (the first version loaded inside the step and waited ~1.5 us eight times per tile — longer than the
-  // main loop of the next tile, which made the GEMM epilogue-bound)
-  uint4 cur[16], nxt[16];
-  auto load_step = [&](int c64, uint4 (&dst)[16]) {
-    const int col0 = n0 + c64 * 64;
+  const float2 g = unpack_bf16(*reinterpret_cast<const uint32_t*>(g_row + col));
+  const float2 u = unpack_bf16(*reinterpret_cast<const uint32_t*>(g_row + N + col));
+  const float d[2] = {bf16_round(v0), bf16_round(v1)}, gv[2] = {g.x, g.y}, uv[2] = {u.x, u.y};
+  float dg[2], du[2];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int col = col0 + i * 8;
-      const bool ok = row_ok && col < N;
-      dst[i] = ok ? *reinterpret_cast<const uint4*>(g_row + col) : make_uint4(0u, 0u, 0u, 0u);
-      dst[8 + i] = ok ? *reinterpret_cast<const uint4*>(g_row + N + col) : make_uint4(0u, 0u, 0u, 0u);
-    }
-  };
-  load_step(0, cur);
-#pragma unroll 1
-  for (int c64 = 0; c64 < BN / 64; ++c64) {
-    const int col0 = n0 + c64 * 64;
-    if (col0 >= N) break;
-    if (c64 + 1 < BN / 64) load_step(c64 + 1, nxt);
-    if (lane == 0) tma_store_wait_read<0>();
-    __syncwarp();
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(t_addr + c64 * 64 + half * 32, r);
-      tmem_wait_ld();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const uint4 gq = cur[half * 4 + g], uq = cur[8 + half * 4 + g];
-        float gv[8], uv[8], dg[8], du[8];
-        const float2 g0 = unpack_bf16(gq.x), g1 = unpack_bf16(gq.y), g2 = unpack_bf16(gq.z), g3 = unpack_bf16(gq.w);
-        const float2 u0 = unpack_bf16(uq.x), u1 = unpack_bf16(uq.y), u2 = unpack_bf16(uq.z), u3 = unpack_bf16(uq.w);
-        gv[0] = g0.x; gv[1] = g0.y; gv[2] = g1.x; gv[3] = g1.y; gv[4] = g2.x; gv[5] = g2.y; gv[6] = g3.x; gv[7] = g3.y;
-        uv[0] = u0.x; uv[1] = u0.y; uv[2] = u1.x; uv[3] = u1.y; uv[4] = u2.x; uv[5] = u2.y; uv[6] = u3.x; uv[7] = u3.y;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          // 128 threads per SM do this arithmetic (the separate pass has 2048): approximate reciprocal (2 ulp, far
-          // below the bf16 rounding of the result) instead of the IEEE division sequence
-          const float d = bf16_round(__uint_as_float(r[g * 8 + j]));
-          const float sg = __fdividef(1.f, 1.f + __expf(-gv[j]));
-          const float silu = gv[j] * sg;
-          du[j] = d * silu;
-          dg[j] = d * uv[j] * (sg * (1.f + gv[j] * (1.f - sg)));
-        }
-        uint4 og, ou;
-        og.x = pack_bf16(dg[0], dg[1]); og.y = pack_bf16(dg[2], dg[3]); og.z = pack_bf16(dg[4], dg[5]); og.w = pack_bf16(dg[6], dg[7]);
-        ou.x = pack_bf16(du[0], du[1]); ou.y = pack_bf16(du[2], du[3]); ou.z = pack_bf16(du[4], du[5]); ou.w = pack_bf16(du[6], du[7]);
-        const int chunk = (half * 4 + g) ^ (lane & 7);            // SWIZZLE_128B, as in epilogue_chunk_staged
-        *reinterpret_cast<uint4*>(buf_g + lane * 128 + chunk * 16) = og;
-        *reinterpret_cast<uint4*>(buf_u + lane * 128 + chunk * 16) = ou;
-      }
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      tma_store_2d(tmC, buf_g, col0, (int)row0);
-      tma_store_2d(tmC, buf_u, N + col0, (int)row0);
-      tma_store_commit();
-    }
-#pragma unroll
-    for (int i = 0; i < 16; ++i) cur[i] = nxt[i];
+  for (int j = 0; j < 2; ++j) {
+    const float sg = __fdividef(1.f, 1.f + __expf(-gv[j]));
+    du[j] = d[j] * (gv[j] * sg);
+    dg[j] = d[j] * uv[j] * (sg * (1.f + gv[j] * (1.f - sg)));
   }
+  bf16* c_row = epi.C + row * epi.ldc;
+  *reinterpret_cast<uint32_t*>(c_row + col) = pack_bf16(dg[0], dg[1]);
+  *reinterpret_cast<uint32_t*>(c_row + N + col) = pack_bf16(du[0], du[1]);
 }
 
 template <bool A_MN, bool B_MN, int BN>
+__device__ __forceinline__ void gemm_mma_stage(float (&acc)[BN / 2], uint32_t a_addr, uint32_t b_addr, int first) {
+#pragma unroll
+  for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
+    const uint64_t da = A_MN ? desc_mnmajor(a_addr, k16, ATOM_BYTES) : desc_kmajor(a_addr, k16);
+    const uint64_t db = B_MN ? desc_mnmajor(b_addr, k16, ATOM_BYTES) : desc_kmajor(b_addr, k16);
+    const int accum = (first && k16 == 0) ? 0 : 1;
+    if constexpr (BN == 256) wgmma_m64n256_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, accum);
+    else wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, accum);
+  }
+}
+
+// CL = 2 (tile_n = 512): a cluster of two CTAs computes a 256 x 256 tile. Each CTA stages its own 128 rows of A and
+// one 128-row half of B, which TMA multicasts into the shared memory of both CTAs: per output element the pair reads B
+// from L2 once instead of twice. A stage slot is refilled only after the math warps of BOTH CTAs have released it
+// (they arrive on the empty barrier of each CTA), since either producer writes into both.
+template <bool A_MN, bool B_MN, int BN, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
-                 const __grid_constant__ CUtensorMap tmC,
-                 int M, int N, int K, GemmSecondSource src2, GemmEpilogue epi, TileCounter* ctr) {
+                 int M, int N, int K, GemmSecondSource src2, GemmEpilogue epi) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint8_t* epi_stage = smem + STAGES * Cfg::STAGE_BYTES;          // 1024-byte aligned (stage sizes are multiples)
-  uint64_t* full = reinterpret_cast<uint64_t*>(epi_stage + EPI_STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* tq_full = tempty + 2;
-  uint64_t* tq_empty = tq_full + GEMM_TQ;
-  volatile int* tile_q = reinterpret_cast<volatile int*>(tq_empty + GEMM_TQ);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(const_cast<int*>(tile_q) + GEMM_TQ);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int num_m = (M + GEMM_BM - 1) / GEMM_BM;
+  const int wg = warp >> 2;
+  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
+  const int first_tile = blockIdx.x / CL, tile_stride = gridDim.x / CL;
+  const int num_m = (M + CL * GEMM_BM - 1) / (CL * GEMM_BM);
   const int num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   const int num_k1 = (K + GEMM_BK - 1) / GEMM_BK;
   const int num_k = num_k1 + (src2.K2 + GEMM_BK - 1) / GEMM_BK;
+  const bool n_grouped = (epi.l2 & 0x40) != 0;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (src2.K2 > 0) {
       tma_prefetch_desc(&tmA2);
       tma_prefetch_desc(&tmB2);
     }
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < STAGES; ++i) {
-        mbar_init(&full[i], 1);
-        mbar_init(&empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tfull[i], 1);
-        mbar_init(&tempty[i], 4);
-      }
-      for (int i = 0; i < GEMM_TQ; ++i) {
-        mbar_init(&tq_full[i], 1);
-        mbar_init(&tq_empty[i], 5);   // MMA thread + 4 epilogue warps
-      }
-      fence_barrier_init();
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 8 * CL);     // lane 0 of each of the 8 math warps (of both CTAs of a pair)
     }
-    __syncwarp();
-    tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
+    fence_barrier_init();
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CL == 2) cluster_sync_all();    // the peer's multicasts and arrives need this CTA's initialised barriers
+  else __syncthreads();
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
-    // The whole warp runs the loop (uniform control flow: coordinates / addresses stay in uniform registers); one
-    // elected lane issues the barrier operations and the bulk-tensor copies (elect.sync is what lets ptxas keep the
-    // single-thread region on the uniform datapath instead of R2UR-converting every operand).
-    {
-      uint32_t leader_lane;
-      const bool leader = elect_one_lane(leader_lane);
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      const uint64_t pol_a = l2_policy(epi.l2 & 3), pol_b = l2_policy((epi.l2 >> 2) & 3);
       int s = 0;
       uint32_t ph = 0;
-      int qs = 0;
-      uint32_t qph = 0;
-      for (int iter = 0;; ++iter) {
-        int t = 0;
-        if (leader) t = epi.dynamic ? (int)atomicAdd(&ctr->next, 1u) : (int)(blockIdx.x + iter * gridDim.x);
-        t = __shfl_sync(0xffffffffu, t, leader_lane);
-        if (t >= num_tiles) t = -1;
-        mbar_wait(&tq_empty[qs], qph ^ 1);
-        if (leader) {
-          tile_q[qs] = t;
-          mbar_arrive(&tq_full[qs]);
-        }
-        if (++qs == GEMM_TQ) { qs = 0; qph ^= 1; }
-        if (t < 0) break;
+      for (int t = first_tile; t < num_tiles; t += tile_stride) {
         int m_blk, n_blk;
-        tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk);
-        const int m0 = m_blk * GEMM_BM, n0 = n_blk * BN;
+        tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, n_grouped);
+        const int m0 = (m_blk * CL + (int)rank) * GEMM_BM, n0 = n_blk * BN;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty[s], ph ^ 1);
           uint8_t* a_dst = smem + s * Cfg::STAGE_BYTES;
@@ -409,438 +209,109 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const bool second = kb >= num_k1;
           const CUtensorMap* mA = second ? &tmA2 : &tmA;
           const CUtensorMap* mB = second ? &tmB2 : &tmB;
-          const int kB = (second ? kb - num_k1 : kb) * GEMM_BK;                      // k index into B
+          const int kB = (second ? kb - num_k1 : kb) * GEMM_BK;                                  // k index into B
           const int kA = second ? kB + (src2.n_sub > 0 ? (n0 / src2.n_sub) * src2.r : 0) : kB;   // into A
-          if (leader) {
-            mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
-            if (A_MN) {
+          mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
+          if (A_MN) {
 #pragma unroll
-              for (int a = 0; a < GEMM_BM / 64; ++a)
-                tma_load_2d(a_dst + a * (GEMM_BK * 128), mA, &full[s], m0 + a * 64, kA);
-            } else {
-              tma_load_2d(a_dst, mA, &full[s], kA, m0);
-            }
+            for (int a = 0; a < GEMM_BM / 64; ++a)
+              tma_load_2d_hint(a_dst + a * ATOM_BYTES, mA, &full[s], m0 + a * 64, kA, pol_a);
+          } else {
+            tma_load_2d_hint(a_dst, mA, &full[s], kA, m0, pol_a);
+          }
+          if (CL == 2) {              // this CTA's half of B, into both CTAs
             if (B_MN) {
 #pragma unroll
-              for (int a = 0; a < BN / 64; ++a)
-                tma_load_2d(b_dst + a * (GEMM_BK * 128), mB, &full[s], n0 + a * 64, kB);
+              for (int a = 2 * (int)rank; a < 2 * (int)rank + 2; ++a)
+                tma_load_2d_mc_hint(b_dst + a * ATOM_BYTES, mB, &full[s], n0 + a * 64, kB, 0x3, pol_b);
             } else {
-              tma_load_2d(b_dst, mB, &full[s], kB, n0);
+              tma_load_2d_mc_hint(b_dst + rank * (128 * 128), mB, &full[s], kB, n0 + 128 * (int)rank, 0x3, pol_b);
             }
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer (whole warp loops, lane 0 issues) ------------------------------
-    {
-      constexpr uint32_t idesc = make_idesc_bf16(GEMM_BM, BN, A_MN, B_MN);
-      const bool leader = elect_one();
-      int s = 0;
-      uint32_t ph = 0;
-      int qs = 0;
-      uint32_t qph = 0;
-      for (int it = 0;; ++it) {
-        mbar_wait(&tq_full[qs], qph);
-        const int t = tile_q[qs];
-        __syncwarp();
-        if (leader) mbar_arrive(&tq_empty[qs]);
-        if (++qs == GEMM_TQ) { qs = 0; qph ^= 1; }
-        if (t < 0) break;
-        const int acc = it & 1;
-        const uint32_t acc_ph = (it >> 1) & 1;
-        mbar_wait(&tempty[acc], acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint32_t b_addr = a_addr + Cfg::A_BYTES;
-          // descriptors of the stage once; per UMMA_K step the start-address field (16-byte units) advances by 2
-          // (K-major: 32 bytes) or 128 (MN-major: 16 rows of 128 bytes)
-          const uint64_t ad0 = A_MN ? desc_mnmajor(a_addr, 0, GEMM_BK) : desc_kmajor(a_addr, 0);
-          const uint64_t bd0 = B_MN ? desc_mnmajor(b_addr, 0, GEMM_BK) : desc_kmajor(b_addr, 0);
-          if (leader) {
+          } else if (B_MN) {
 #pragma unroll
-            for (int k16 = 0; k16 < GEMM_BK / 16; ++k16)
-              umma_ss(d_tmem, ad0 + (uint64_t)(k16 * (A_MN ? 128 : 2)), bd0 + (uint64_t)(k16 * (B_MN ? 128 : 2)), idesc,
-                      (kb > 0 || k16 > 0) ? 1u : 0u);
-            umma_commit(&empty[s]);  // smem slot is free once these MMAs have read it
-            if (kb == num_k - 1) umma_commit(&tfull[acc]);
+            for (int a = 0; a < BN / 64; ++a)
+              tma_load_2d_hint(b_dst + a * ATOM_BYTES, mB, &full[s], n0 + a * 64, kB, pol_b);
+          } else {
+            tma_load_2d_hint(b_dst, mB, &full[s], kB, n0, pol_b);
           }
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
   } else {
-    // ------------------------------ epilogue ------------------------------
-    const int quad = warp & 3;
-    const int row_in_tile = quad * 32 + lane;
-    uint8_t* warp_stage = epi_stage + quad * 2 * EPI_BUF_BYTES;
-    int buf_sel = 0;
-    int qs = 0;
-    uint32_t qph = 0;
-    if (lane == 0 && epi.tma_store) tma_prefetch_desc(&tmC);
-    for (int it = 0;; ++it) {
-      mbar_wait(&tq_full[qs], qph);
-      const int t = tile_q[qs];
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tq_empty[qs]);
-      if (++qs == GEMM_TQ) { qs = 0; qph ^= 1; }
-      if (t < 0) break;
+    // ------------------------------ MMA + epilogue: 64 rows per warpgroup ------------------------------
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;                                  // rows [64*cw, 64*cw + 64) of the tile
+    const int g = lane >> 2, tq = lane & 3;
+    float acc[BN / 2];
+    int s = 0;
+    uint32_t ph = 0;
+    auto release = [&](int slot) {
+      mbar_arrive(&empty[slot]);
+      if (CL == 2) mbar_arrive_cluster(&empty[slot], rank ^ 1);
+    };
+    for (int t = first_tile; t < num_tiles; t += tile_stride) {
       int m_blk, n_blk;
-      tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk);
-      const int acc = it & 1;
-      const uint32_t acc_ph = (it >> 1) & 1;
-      mbar_wait(&tfull[acc], acc_ph);
-      tc_fence_after();
-      const long long row = (long long)m_blk * GEMM_BM + row_in_tile;
-      const bool row_ok = row < M;
-      const uint32_t t_addr = tmem_base + acc * BN + ((uint32_t)(quad * 32) << 16);
-      if (epi.tma_store && !(epi.debug & 3)) {
-        if (epi.glu)
-          epilogue_tile_glu<BN>(t_addr, (long long)m_blk * GEMM_BM + quad * 32, row, row_ok, n_blk * BN, N, epi, &tmC,
-                                warp_stage, lane);
-        else
-        epilogue_tile_tma<BN>(t_addr, (long long)m_blk * GEMM_BM + quad * 32, row, row_ok, n_blk * BN, N, epi, &tmC,
-                              warp_stage, lane, buf_sel);
-      } else {
-        bf16* c_row = epi.C + row * epi.ldc;
-        const bf16* r_row = epi.residual ? epi.residual + row * epi.ldr : nullptr;
-#pragma unroll 1
-        for (int ch = 0; ch < BN / 32; ++ch) {
-          if (epi.debug & 2) break;
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(t_addr + ch * 32, r);
-          tmem_wait_ld();
-          const int col0 = n_blk * BN + ch * 32;
-          if (row_ok && col0 < N && !(epi.debug & 1)) epilogue_chunk(r, col0, N, c_row, r_row, epi);
-        }
+      tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, n_grouped);
+      int prev = -1;
+      for (int kb = 0; kb < num_k; ++kb) {
+        mbar_wait(&full[s], ph);
+        const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * ATOM_BYTES;   // 64 rows / 2nd M atom
+        const uint32_t b_addr = smem_u32(smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+        reg_fence(acc);
+        wgmma_fence();
+        gemm_mma_stage<A_MN, B_MN, BN>(acc, a_addr, b_addr, kb == 0);
+        wgmma_commit();
+        wgmma_wait<1>();              // the previous stage's MMAs are complete: hand its slot back to the producer
+        reg_fence(acc);
+        if (prev >= 0 && lane == 0) release(prev);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-    }
-    if (lane == 0 && epi.tma_store) tma_store_wait_all<0>();     // staging smem must outlive the last bulk stores
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-  if (threadIdx.x == 0) {
-    const unsigned int d = atomicAdd(&ctr->done, 1u);
-    if (d == gridDim.x - 1) {   // every CTA has drawn its last index: re-arm for the next launch
-      ctr->next = 0;
-      ctr->done = 0;
-      __threadfence();
-    }
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// 2-CTA variant (cta_group::2): a cluster of two CTAs on one TPC computes a 256 x 256 tile with one
-// UMMA (M=256, N=256, K=16) per step issued by the leader CTA. Each CTA stages only its own 128
-// rows of A and its own 128-row half of B (the tensor cores read the peer's half through the pair's
-// shared-memory link), which halves the shared-memory traffic per SM and allows a 6-stage ring.
-// ------------------------------------------------------------------------------------------------
-constexpr int GEMM2_STAGES = 6;
-constexpr uint32_t GEMM2_A_BYTES = 128 * GEMM_BK * 2;
-constexpr uint32_t GEMM2_B_BYTES = 128 * GEMM_BK * 2;
-constexpr uint32_t GEMM2_STAGE_BYTES = GEMM2_A_BYTES + GEMM2_B_BYTES;
-constexpr uint32_t GEMM2_SMEM_BYTES = GEMM2_STAGES * GEMM2_STAGE_BYTES + EPI_STAGE_BYTES + 512 + 1024;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta));
-  return r;
-}
-
-template <bool A_MN, bool B_MN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm2_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
-                  const __grid_constant__ CUtensorMap tmC,
-                  int M, int N, int K, GemmSecondSource src2, GemmEpilogue epi, TileCounter* ctr) {
-  constexpr int STAGES = GEMM2_STAGES;
-  constexpr int BN = 256;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* epi_stage = smem + STAGES * GEMM2_STAGE_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(epi_stage + EPI_STAGE_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* tq_full = tempty + 2;            // tile index landed in this CTA's queue slot
-  uint64_t* tq_empty = tq_full + GEMM_TQ;    // (leader's copy) every consumer of both CTAs has read the slot
-  volatile int* tile_q = reinterpret_cast<volatile int*>(tq_empty + GEMM_TQ);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(const_cast<int*>(tile_q) + GEMM_TQ);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = cluster_ctarank();
-  const int num_clusters = gridDim.x >> 1;
-  const int num_m = (M + 255) / 256;
-  const int num_n = (N + BN - 1) / BN;
-  const int num_tiles = num_m * num_n;
-  const int num_k1 = (K + GEMM_BK - 1) / GEMM_BK;
-  const int num_k = num_k1 + (src2.K2 + GEMM_BK - 1) / GEMM_BK;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < STAGES; ++i) {
-        mbar_init(&full[i], 2);    // leader: own arrive.expect_tx + peer's remote arrive
-        mbar_init(&empty[i], 1);   // multicast tcgen05.commit
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tfull[i], 1);   // multicast tcgen05.commit
-        mbar_init(&tempty[i], 8);  // 4 epilogue warps of each CTA arrive on the leader's barrier
-      }
-      for (int i = 0; i < GEMM_TQ; ++i) {
-        mbar_init(&tq_full[i], 1);    // one arrive by the leader's producer (local / remote)
-        mbar_init(&tq_empty[i], 10);  // leader: MMA + 4 epilogue warps; peer: producer + 4 epilogue warps
-      }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc_2sm<512>(tmem_slot);
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ------------------------------ TMA producer (both CTAs); the leader CTA's also schedules tiles ------------------
-    // whole warp loops, one elected lane issues (see gemm_bf16_kernel)
-    {
-      uint32_t leader_lane;
-      const bool leader = elect_one_lane(leader_lane);
-      int s = 0;
-      uint32_t ph = 0;
-      int qs = 0;
-      uint32_t qph = 0;
-      for (int iter = 0;; ++iter) {
-        int t = 0;
-        if (cta_rank == 0) {
-          if (leader) t = epi.dynamic ? (int)atomicAdd(&ctr->next, 1u) : (int)((blockIdx.x >> 1) + iter * num_clusters);
-          t = __shfl_sync(0xffffffffu, t, leader_lane);
-          if (t >= num_tiles) t = -1;
-          mbar_wait_cluster(&tq_empty[qs], qph ^ 1);
-          if (leader) {
-            tile_q[qs] = t;
-            st_shared_cluster_u32(const_cast<int*>(&tile_q[qs]), 1, (uint32_t)t);
-            mbar_arrive(&tq_full[qs]);
-            mbar_arrive_cluster_release(&tq_full[qs], 1);
-          }
-        } else {
-          mbar_wait_cluster(&tq_full[qs], qph);
-          t = tile_q[qs];
-          __syncwarp();
-          if (leader) mbar_arrive_cluster_release(&tq_empty[qs], 0);
-        }
-        if (++qs == GEMM_TQ) { qs = 0; qph ^= 1; }
-        if (t < 0) break;
-        int m_blk, n_blk;
-        tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, (epi.l2 & 0x40) != 0);
-        const int m0 = m_blk * 256 + (int)cta_rank * 128;
-        const int n0 = n_blk * BN + (int)cta_rank * 128;
-        const uint64_t pol_a = l2_policy(epi.l2 & 3), pol_b = l2_policy((epi.l2 >> 2) & 3);
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&empty[s], ph ^ 1);
-          uint8_t* a_dst = smem + s * GEMM2_STAGE_BYTES;
-          uint8_t* b_dst = a_dst + GEMM2_A_BYTES;
-          const uint32_t leader_full = mapa_u32(smem_u32(&full[s]), 0);
-          const bool second = kb >= num_k1;
-          const CUtensorMap* mA = second ? &tmA2 : &tmA;
-          const CUtensorMap* mB = second ? &tmB2 : &tmB;
-          const int kB = (second ? kb - num_k1 : kb) * GEMM_BK;
-          const int kA = second ? kB + (src2.n_sub > 0 ? ((n_blk * BN) / src2.n_sub) * src2.r : 0) : kB;
-          if (leader) {
-            if (cta_rank == 0) mbar_arrive_expect_tx(&full[s], 2 * GEMM2_STAGE_BYTES);
-            else mbar_arrive_cluster(&full[s], 0);
-            if (A_MN) {
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (lane == 0) release(prev);
+      if (epi.debug & 1) continue;
+      const long long row0 = (long long)(m_blk * CL + (int)rank) * GEMM_BM + cw * 64 + (warp & 3) * 16 + g;
 #pragma unroll
-              for (int a = 0; a < 2; ++a)
-                tma_load_2d_2sm_hint(a_dst + a * (GEMM_BK * 128), mA, leader_full, m0 + a * 64, kA, pol_a);
-            } else {
-              tma_load_2d_2sm_hint(a_dst, mA, leader_full, kA, m0, pol_a);
-            }
-            if (B_MN) {
+      for (int h = 0; h < 2; ++h) {
+        const long long row = row0 + h * 8;
+        if (row >= M) continue;
 #pragma unroll
-              for (int a = 0; a < 2; ++a)
-                tma_load_2d_2sm_hint(b_dst + a * (GEMM_BK * 128), mB, leader_full, n0 + a * 64, kB, pol_b);
-            } else {
-              tma_load_2d_2sm_hint(b_dst, mB, leader_full, kB, n0, pol_b);
-            }
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+        for (int i = 0; i < BN / 8; ++i) {
+          const int col = n_blk * BN + i * 8 + tq * 2;
+          if (col >= N) continue;
+          if (epi.glu) epilogue_pair_glu(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], row, col, N, epi);
+          else epilogue_pair(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], row, col, epi);
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer (leader CTA only; whole warp loops, elected lane issues) ------------
-    if (cta_rank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(256, BN, A_MN, B_MN);
-      const bool leader = elect_one();
-      int s = 0;
-      uint32_t ph = 0;
-      int qs = 0;
-      uint32_t qph = 0;
-      for (int it = 0;; ++it) {
-        mbar_wait(&tq_full[qs], qph);
-        const int t = tile_q[qs];
-        __syncwarp();
-        if (leader) mbar_arrive(&tq_empty[qs]);
-        if (++qs == GEMM_TQ) { qs = 0; qph ^= 1; }
-        if (t < 0) break;
-        const int acc = it & 1;
-        const uint32_t acc_ph = (it >> 1) & 1;
-        mbar_wait(&tempty[acc], acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * GEMM2_STAGE_BYTES);
-          const uint32_t b_addr = a_addr + GEMM2_A_BYTES;
-          const uint64_t ad0 = A_MN ? desc_mnmajor(a_addr, 0, GEMM_BK) : desc_kmajor(a_addr, 0);
-          const uint64_t bd0 = B_MN ? desc_mnmajor(b_addr, 0, GEMM_BK) : desc_kmajor(b_addr, 0);
-          if (leader) {
-#pragma unroll
-            for (int k16 = 0; k16 < GEMM_BK / 16; ++k16)
-              umma_ss_2sm(d_tmem, ad0 + (uint64_t)(k16 * (A_MN ? 128 : 2)), bd0 + (uint64_t)(k16 * (B_MN ? 128 : 2)),
-                          idesc, (kb > 0 || k16 > 0) ? 1u : 0u);
-            umma_commit_2sm(&empty[s], 0x3);
-            if (kb == num_k - 1) umma_commit_2sm(&tfull[acc], 0x3);
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ------------------------------ epilogue (both CTAs) ------------------------------
-    const int quad = warp & 3;
-    const int row_in_tile = (int)cta_rank * 128 + quad * 32 + lane;
-    uint8_t* warp_stage = epi_stage + quad * 2 * EPI_BUF_BYTES;
-    int buf_sel = 0;
-    int qs = 0;
-    uint32_t qph = 0;
-    if (lane == 0 && epi.tma_store) tma_prefetch_desc(&tmC);
-    for (int it = 0;; ++it) {
-      if (cta_rank == 0) mbar_wait(&tq_full[qs], qph);
-      else mbar_wait_cluster(&tq_full[qs], qph);
-      const int t = tile_q[qs];
-      __syncwarp();
-      if (lane == 0) {
-        if (cta_rank == 0) mbar_arrive(&tq_empty[qs]);
-        else mbar_arrive_cluster_release(&tq_empty[qs], 0);
-      }
-      if (++qs == GEMM_TQ) { qs = 0; qph ^= 1; }
-      if (t < 0) break;
-      int m_blk, n_blk;
-      tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, (epi.l2 & 0x40) != 0);
-      const int acc = it & 1;
-      const uint32_t acc_ph = (it >> 1) & 1;
-      mbar_wait(&tfull[acc], acc_ph);
-      tc_fence_after();
-      const long long row = (long long)m_blk * 256 + row_in_tile;
-      const bool row_ok = row < M;
-      const uint32_t t_addr = tmem_base + acc * BN + ((uint32_t)(quad * 32) << 16);
-      if (epi.tma_store && !(epi.debug & 3)) {
-        if (epi.glu)
-          epilogue_tile_glu<BN>(t_addr, (long long)m_blk * 256 + (int)cta_rank * 128 + quad * 32, row, row_ok, n_blk * BN,
-                                N, epi, &tmC, warp_stage, lane);
-        else
-        epilogue_tile_tma<BN>(t_addr, (long long)m_blk * 256 + (int)cta_rank * 128 + quad * 32, row, row_ok, n_blk * BN,
-                              N, epi, &tmC, warp_stage, lane, buf_sel);
-      } else {
-        bf16* c_row = epi.C + row * epi.ldc;
-        const bf16* r_row = epi.residual ? epi.residual + row * epi.ldr : nullptr;
-#pragma unroll 1
-        for (int ch = 0; ch < BN / 32; ++ch) {
-          if (epi.debug & 2) break;
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(t_addr + ch * 32, r);
-          tmem_wait_ld();
-          const int col0 = n_blk * BN + ch * 32;
-          if (row_ok && col0 < N && !(epi.debug & 1)) epilogue_chunk(r, col0, N, c_row, r_row, epi);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (cta_rank == 0) mbar_arrive(&tempty[acc]);
-        else mbar_arrive_cluster(&tempty[acc], 0);
-      }
-    }
-    if (lane == 0 && epi.tma_store) tma_store_wait_all<0>();     // staging smem must outlive the last bulk stores
   }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
-  }
-  if (threadIdx.x == 0 && cta_rank == 0) {
-    const unsigned int d = atomicAdd(&ctr->done, 1u);
-    if (d == (unsigned int)num_clusters - 1) {
-      ctr->next = 0;
-      ctr->done = 0;
-      __threadfence();
-    }
-  }
+  if (CL == 2) cluster_sync_all();    // the peer may still multicast into / arrive on this CTA's shared memory
 }
 
-template <bool A_MN, bool B_MN>
-static int launch_gemm2(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2,
-                        const CUtensorMap& tmB2, const CUtensorMap& tmC, int M, int N, int K,
-                        const GemmSecondSource& src2, const GemmEpilogue& epi, cudaStream_t stream) {
-  auto kern = gemm2_bf16_kernel<A_MN, B_MN>;
-  B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)GEMM2_SMEM_BYTES));
-  const int num_tiles = ((M + 255) / 256) * ((N + 255) / 256);
-  int clusters = num_sms() / 2;
-  if (num_tiles < clusters) clusters = num_tiles;
-  if (!g_counter_pool) B200_CHECK_CUDA(cudaGetSymbolAddress((void**)&g_counter_pool, g_tile_counters));
-  TileCounter* ctr = g_counter_pool + (g_launch_seq++ & 63);
-  kern<<<clusters * 2, GEMM_THREADS, GEMM2_SMEM_BYTES, stream>>>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, ctr);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <bool A_MN, bool B_MN, int BN>
+template <bool A_MN, bool B_MN, int BN, int CL>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2,
-                       const CUtensorMap& tmB2, const CUtensorMap& tmC, int M, int N, int K,
-                       const GemmSecondSource& src2, const GemmEpilogue& epi, cudaStream_t stream) {
+                       const CUtensorMap& tmB2, int M, int N, int K, const GemmSecondSource& src2,
+                       const GemmEpilogue& epi, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<A_MN, B_MN, BN>;
+  auto kern = gemm_bf16_kernel<A_MN, B_MN, BN, CL>;
   B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)Cfg::SMEM_BYTES));
-  const int num_tiles = ((M + GEMM_BM - 1) / GEMM_BM) * ((N + BN - 1) / BN);
-  const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-  if (!g_counter_pool) B200_CHECK_CUDA(cudaGetSymbolAddress((void**)&g_counter_pool, g_tile_counters));
-  TileCounter* ctr = g_counter_pool + (g_launch_seq++ & 63);
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, ctr);
-  B200_CHECK_CUDA(cudaGetLastError());
+  const int num_tiles = ((M + CL * GEMM_BM - 1) / (CL * GEMM_BM)) * ((N + BN - 1) / BN);
+  const int slots = num_sms() / CL;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((num_tiles < slots ? num_tiles : slots) * CL);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = CL;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmA2, tmB2, M, N, K, src2, epi));
   return 0;
 }
 
@@ -867,30 +338,26 @@ using namespace b200;
 
 static int g_group_m = 16;
 static int g_debug = 0;
-static int g_tma_store = 1;   // C through swizzled smem + cp.async.bulk.tensor stores (rlaifv_gemm_set_tuning debug bit 8 = off)
 extern "C" int rlaifv_gemm_set_tuning(int group_m, int debug) {
   if (group_m > 0) g_group_m = group_m;
-  g_debug = debug & 7;
-  g_tma_store = (debug & 8) ? 0 : 1;
+  g_debug = debug & 1;
   return 0;
 }
-// L2 policy of the CTA-pair kernel (GemmEpilogue::l2); the 1-CTA kernel ignores the load policies and the raster bit.
-// l2 < 0 (default): chosen per launch by l2_auto_policy() below; l2 >= 0: the given bits for every launch.
+// L2 policy of the operand loads and the tile raster (GemmEpilogue::l2; bits 4-5, the C-store hint, are accepted and
+// ignored: C leaves through ordinary stores). l2 < 0 (default): chosen per launch by l2_auto_policy() below; l2 >= 0:
+// the given bits for every launch.
 static int g_l2 = -1;
 extern "C" int rlaifv_gemm_set_l2(int l2) {
   g_l2 = l2 < 0 ? -1 : (l2 & 0x7f);
   return 0;
 }
-// Long-K launches (dgrad / wgrad / down projection: K = 11008 .. 22016) have 256-row operand panels of 6-11 MB; with
-// the default raster (16 row blocks per group) the panels one wave of 74 CTA pairs touches (130+ MB) fall out of the
-// L2 before the next wave needs them again and the launch reads 4-5x its operands from DRAM (ncu: dgrad qkv 3.2 GB vs
-// 0.55 GB of operands). Grouping along the SHORTER tile dimension keeps the smaller operand's panels resident while the
-// larger one streams: DRAM reads = (streamed operand) x ceil(blocks / group) + (resident operand), and the resident set
-// (group x panel) has to stay well under the L2: 8 panels up to K = 16384, 4 beyond. The resident operand's TMA loads
-// carry evict_last, the streamed one's evict_first. Measured (tools/gpu_gemm_l2_sweep.py, profiles/r02u_*): dgrad qkv
-// 3.20 -> 1.65 GB, wgrad qkv 4.32 -> 2.27 GB, dgrad gate|up 8.28 -> 4.8-5.1 GB per launch; the config-(b) step 665.5 ->
-// 654.1 ms in-process (profiles/r02u_step_ab_l2_policy.log). The raster is what pays: hints off, group 4 / 6 / 8 all
-// land within 0.1 % of each other at step level (profiles/r02u_step_ab_l2_variants.log). Results are bit-identical.
+// Long-K launches (dgrad / wgrad / down projection: K = 11008 .. 22016) have operand panels of several MB per tile
+// row or column; with the default raster (16 row blocks per group) the panels one wave of CTAs touches can fall out of
+// the L2 before the next wave needs them again, and the launch then reads its operands from DRAM several times over.
+// Grouping along the SHORTER tile dimension keeps the smaller operand's panels resident while the larger one streams:
+// DRAM reads = (streamed operand) x ceil(blocks / group) + (resident operand), and the resident set (group x panel)
+// has to stay well under the L2: 8 panels up to K = 16384, 4 beyond. The resident operand's TMA loads carry
+// evict_last, the streamed one's evict_first. Tile order and cache hints never change a bit of the result.
 static void l2_auto_policy(int M, int N, int K, int* l2, int* group) {
   if (K < 8192) return;                                    // short K: panels are small, the default raster is the best
   const bool n_grouped = N < M;
@@ -898,13 +365,6 @@ static void l2_auto_policy(int M, int N, int K, int* l2, int* group) {
   *l2 = n_grouped ? (0x40 | 1 | (2 << 2))                  // column blocks grouped: B resident, A streams
                   : (2 | (1 << 2));                        // row blocks grouped: A resident, B streams
 }
-// auto-selection policy for tile_n = 0: 0 never, 1 whenever the problem is large, 2 (default) where measured faster
-static int g_enable_2cta = 2;
-extern "C" int rlaifv_gemm_set_2cta(int enable) {
-  g_enable_2cta = enable;
-  return 0;
-}
-
 // C ABI — see include/rlaifv_b200.h for the contract.
 // EXPERIMENTAL, off by default (rlaifv_gemm_set_split_k): long-K launches without bias / activation / residual
 // (dgrad, wgrad) run as `n` passes over K slices, passes 2.. with C += — each pass's operand slabs then fit the L2
@@ -952,13 +412,14 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
   B200_REQUIRE(((uintptr_t)C & 15) == 0, "gemm: C not 16-byte aligned");
   int bn = tile_n;
   if (bn == 0) {
+    // the 128 x 256 tile halves the B-operand shared-memory traffic per output element of the 128 x 128 one, and the
+    // CTA-pair form halves B's L2 reads again; each is taken once there are enough of its tiles to fill the SMs. Measured
+    // on an H100 SXM (700 W) on the LLaVA-7B layer shapes at M = 9080: the pair is 1-3 % faster than the single-CTA
+    // 128 x 256 tile on every forward, dgrad and wgrad shape, with bit-identical results.
     const long long tiles256 = (long long)((M + 127) / 128) * ((N + 255) / 256);
     const long long tiles2 = (long long)((M + 255) / 256) * ((N + 255) / 256);
-    // measured on B200 in one process (tools/gpu_gemm_pair_ab.py, profiles/r01_gemm_pair_ab.log): the CTA-pair
-    // kernel is 5-10% faster than the 1-CTA kernel on every layer shape (the part is power-limited and the
-    // pair halves the B-operand shared-memory traffic), so policy 2 (default) takes it for any large problem.
-    if (N >= 256 && g_enable_2cta != 0 && tiles2 >= 64) bn = 512;
-    else bn = (N >= 256 && tiles256 >= 120) ? 256 : 128;
+    if (N >= 256 && tiles2 >= num_sms() / 2) bn = 512;
+    else bn = (N >= 256 && tiles256 >= num_sms()) ? 256 : 128;
   }
   B200_REQUIRE(bn == 128 || bn == 256 || bn == 512, "gemm: tile_n must be 0, 128, 256 or 512 (2-CTA 256x256)");
   GemmSecondSource src2;
@@ -985,19 +446,7 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
     rc = operand_tmap(&tmB2, B2, ldb2, b_mn_major != 0, N, K2, bn == 512 ? 128 : bn);
     if (rc) return rc;
   }
-  // C tensor map for the TMA-store epilogue: [M rows][N cols], row stride ldc, box = 64 columns x 32 rows (one
-  // epilogue warp's slab), SWIZZLE_128B like the operand tiles
-  CUtensorMap tmC = tmA;
-  int use_tma_store = g_tma_store;
-  if (use_tma_store) {
-    uint64_t cdims[2] = {(uint64_t)(glu ? 2 * N : N), (uint64_t)M};      // swiglu_bwd epilogue: C is [M, 2F]
-    uint64_t cstr[1] = {(uint64_t)ldc * 2};
-    uint32_t cbox[2] = {64, 32};
-    if (make_tmap_bf16(&tmC, C, 2, cdims, cstr, cbox) != 0) use_tma_store = 0;    // odd view: direct stores instead
-  }
-  B200_REQUIRE(!glu || use_tma_store, "gemm (swiglu_bwd epilogue): needs the TMA-store epilogue (C view not mappable)");
   GemmEpilogue epi;
-  epi.tma_store = use_tma_store;
   epi.C = (bf16*)C;
   epi.ldc = ldc;
   epi.bias = (const bf16*)bias;
@@ -1009,29 +458,22 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
   epi.glu = (const bf16*)glu;
   epi.ld_glu = ld_glu;
   epi.group_m = g_group_m;
-  epi.debug = g_debug & 3;
-  epi.dynamic = (g_debug & 4) ? 0 : 1;
+  epi.debug = g_debug;
   epi.l2 = 0;
-  if (bn == 512) {
-    if (g_l2 < 0) l2_auto_policy(M, N, K, &epi.l2, &epi.group_m);
-    else epi.l2 = g_l2;
-  } else if (g_l2 > 0) {
-    epi.l2 = g_l2 & 0x30;
-  }
+  if (g_l2 < 0) l2_auto_policy(M, N, K, &epi.l2, &epi.group_m);
+  else epi.l2 = g_l2 & 0x4f;
   cudaStream_t st = (cudaStream_t)stream;
-  if (bn == 512) {
-    if (!a_mn_major && !b_mn_major) return launch_gemm2<false, false>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st);
-    if (!a_mn_major && b_mn_major) return launch_gemm2<false, true>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st);
-    return launch_gemm2<true, true>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st);
-  }
   if (!a_mn_major && !b_mn_major)
-    return bn == 256 ? launch_gemm<false, false, 256>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st)
-                     : launch_gemm<false, false, 128>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st);
+    return bn == 512 ? launch_gemm<false, false, 256, 2>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
+         : bn == 256 ? launch_gemm<false, false, 256, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
+                     : launch_gemm<false, false, 128, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st);
   if (!a_mn_major && b_mn_major)
-    return bn == 256 ? launch_gemm<false, true, 256>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st)
-                     : launch_gemm<false, true, 128>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st);
-  return bn == 256 ? launch_gemm<true, true, 256>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st)
-                   : launch_gemm<true, true, 128>(tmA, tmB, tmA2, tmB2, tmC, M, N, K, src2, epi, st);
+    return bn == 512 ? launch_gemm<false, true, 256, 2>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
+         : bn == 256 ? launch_gemm<false, true, 256, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
+                     : launch_gemm<false, true, 128, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st);
+  return bn == 512 ? launch_gemm<true, true, 256, 2>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
+       : bn == 256 ? launch_gemm<true, true, 256, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
+                   : launch_gemm<true, true, 128, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st);
 }
 
 extern "C" int rlaifv_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb,

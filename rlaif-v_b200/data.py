@@ -7,7 +7,7 @@
   PreferenceInferenceDataset / InferenceSampler / get_multimodal_sample_logps /
   write_logp_to_preference_parquet / inference_logp
                                   muffin/eval/muffin_inference_logp.py:55-79,117-164,213-344
-      — the frozen-reference log-prob pre-pass (SURVEY.md §8f-1).  Here it runs on the same B200
+      — the frozen-reference log-prob pre-pass (SURVEY.md §8f-1).  Here it runs on the same H100
         forward kernels as training: win and rej of a pair in ONE forward sharing the encoded image
         (the reference runs 2 forwards per pair and encodes the image twice), batched, and writes the
         identical on-disk contract: column `logps` = json.dumps({'logps': [win_sum, win_avg,

@@ -10,10 +10,10 @@ num_classes=0, dynamic_img_size=True, dynamic_img_pad=True)` with the last block
 on every token.  (The tests' CPU restatement of it lives under oracle/; timm is absent from the image, so that
 restatement is parity-unpinned.)
 
-B200 mapping — nothing here is a new kernel family; the tower is built from the library's existing pieces:
-  * every contraction is the tcgen05 GEMM (bias / residual epilogues, dgrad, wgrad straight into the flat bf16
+Kernel mapping — nothing here is a new kernel family; the tower is built from the library's existing pieces:
+  * every contraction is the wgmma GEMM (bias / residual epilogues, dgrad, wgrad straight into the flat bf16
     gradient bucket);
-  * attention is the TMEM-resident non-causal kernel pair (d = 128).  The model's head width is 112, so the fused qkv
+  * attention is the register-resident non-causal wgmma kernel pair (d = 128).  The model's head width is 112, so the fused qkv
     / proj weights are stored PADDED per head to 128 (16 zero rows per head in `qkv`, 16 zero columns per head in
     `proj`): q.k^T and P.V are unchanged by zero padding, every gradient that lands on a padded element is exactly
     zero (dQ_pad = dS.K_pad = 0, dK_pad = dS^T.Q_pad = 0, dV_pad = P^T.dO_pad with dO_pad = d(att).Wo_pad^T = 0), and

@@ -28,8 +28,6 @@ _SIGNATURES = {
                               c_void_p],
     "rlaifv_gemm_bf16_swiglu_bwd": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_int, c_void_p,
                                     c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_void_p],
-    "rlaifv_gemm_set_2cta": [c_int],
-    "rlaifv_attention_set_variant": [c_int],
     "rlaifv_attention_bwd_split": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p,
                                    c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                    c_int, c_int, c_float, c_void_p],

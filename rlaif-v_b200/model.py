@@ -1,4 +1,4 @@
-"""LLaVA-1.5 DPO policy on the B200 kernels: parameter storage + hand-written forward / backward.
+"""LLaVA-1.5 DPO policy on the H100 kernels: parameter storage + hand-written forward / backward.
 
 Mirrors what the reference executes in `get_beta_and_logps(..., is_llava15=True)`
 (muffin/train/trainers.py:205-231): CLIP tower (frozen, llava/model/multimodal_encoder/clip_encoder.py:46-58)
@@ -416,7 +416,7 @@ class LlavaDPOPolicy:
 
     def _lin_fwd(self, i, group, x, out, residual=None, ls=None):
         """out = x @ W^T (+ residual). LoRA: t = s * x @ A^T (all sub-linears' lora_A stacked), then ONE GEMM
-        accumulates x @ W^T and t_j @ B_j^T in the same TMEM tile (rlaifv_gemm_bf16_dual)."""
+        accumulates x @ W^T and t_j @ B_j^T in the same accumulator tile (rlaifv_gemm_bf16_dual)."""
         W = self.store.p[f"l{i}.{group}"]
         if self.lora is None:
             return ops.gemm(x, W, out, residual=residual)

@@ -1,4 +1,4 @@
-"""OmniLMM-12B DPO policy (BASELINE config d; SURVEY.md §8 a13) on the B200 kernels: EVA vision tower (eva_tower.py,
+"""OmniLMM-12B DPO policy (BASELINE config d; SURVEY.md §8 a13) on the H100 kernels: EVA vision tower (eva_tower.py,
 trainable) -> perceiver resampler -> in-place <im_patch> splice -> Mistral decoder (grouped-query attention) ->
 per-token log-prob gather, and the backward of all of it.
 

@@ -1,5 +1,5 @@
 """Perceiver resampler of OmniLMM-12B (BASELINE config d; SURVEY.md §8 a13) on the CUDA library — forward and
-backward, all arithmetic in the sm_100a kernels (tcgen05 GEMMs, cross-attention with S/O in TMEM, LayerNorm fwd/bwd).
+backward, all arithmetic in the sm_90a kernels (wgmma GEMMs, cross-attention with S/O in registers, LayerNorm fwd/bwd).
 
 Mirrors `Resampler` of omnilmm/model/resampler.py:93-168 (same parameter names, so `state_dict()` keys line up with
 `model.resampler.*` of an OmniLMM checkpoint):

@@ -103,7 +103,7 @@ class TrainingArguments:                   # muffin/train/train_llava15.py:72-10
     dataloader_num_workers: int = 0
     seed: int = 42
     local_rank: int = -1
-    micro_pairs: Optional[int] = None      # B200 engine knob: pairs per micro-batch (None = whole batch)
+    micro_pairs: Optional[int] = None      # engine knob: pairs per micro-batch (None = whole batch)
     # muffin/train/train_llava15_lora.py:112-117
     lora_enable: bool = False
     lora_r: int = 64

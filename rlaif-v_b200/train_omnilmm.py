@@ -11,9 +11,9 @@ reference-log-prob dataset of the LLaVA recipe, and ZeRO (script/zero3.json for 
         --task DPO --dpo_beta 0.1 --deepspeed ./script/zero3.json --bf16 True ...
 
 Flags are those of train_llava15 (same three argument groups) plus --num_query / --image_size / --tune_clip.
-ZeRO: `--deepspeed` may name a stage-2 or stage-3 config; the engine runs its native ZeRO-2 either way — with 180 GB per
-GPU the 23 GB of bf16 parameters replicate, and what ZeRO-3 would add (parameter sharding) buys nothing at 8 GPUs
-(DESIGN.md §6c has the memory plan).
+ZeRO: `--deepspeed` may name a stage-2 or stage-3 config; the engine runs its native ZeRO-2 either way: the 23 GB of
+bf16 parameters replicate on every GPU and the fp32 optimizer state is sharded (186 GB of training state in all: at
+least 4 80 GB GPUs).
 """
 import dataclasses
 import json

@@ -1,5 +1,5 @@
 #!/bin/bash
-# B200 launch of LLaVA-1.5-7B DPO: every flag of the reference recipe (its script/train/llava15_train.sh) is accepted
+# Launch of LLaVA-1.5-7B DPO: every flag of the reference recipe (its script/train/llava15_train.sh) is accepted
 # with the same meaning; the launcher is torchrun (one process per GPU, NCCL over NVLink) and ZeRO-2 is native.
 export PYTHONPATH=$PYTHONPATH:`realpath .`
 task_name=llava15_7b_DPO

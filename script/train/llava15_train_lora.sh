@@ -1,5 +1,5 @@
 #!/bin/bash
-# B200 launch of LLaVA-1.5-7B LoRA-DPO (r=64, alpha=16, dropout 0.05): the flags of the reference recipe (its
+# Launch of LLaVA-1.5-7B LoRA-DPO (r=64, alpha=16, dropout 0.05): the flags of the reference recipe (its
 # script/train/llava15_train_lora.sh), torchrun launcher, native ZeRO-2 over the adapter + projector buckets.
 export PYTHONPATH=$PYTHONPATH:`realpath .`
 task_name=llava15_7b_DPO

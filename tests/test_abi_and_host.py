@@ -36,15 +36,15 @@ def test_library_exports_every_declared_symbol():
     assert handle.rlaifv_last_error() is not None
 
 
-def test_sass_is_blackwell_native():
+def test_sass_is_hopper_native():
     so = os.path.join(REPO, "rlaif-v_b200", "librlaifv_b200.so")
     if not os.path.exists(so):
         pytest.skip("library not built")
     sass = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass          # tcgen05.mma
+    assert "HGMMA" in sass            # wgmma.mma_async
     assert "UTMALDG" in sass          # TMA loads
-    assert "LDTM" in sass             # tcgen05.ld
-    assert "HMMA." not in sass.replace("UTCHMMA", "")   # no legacy mma.sync path
+    assert "SYNCS" in sass            # mbarrier
+    assert "HMMA." not in sass        # no legacy mma.sync path
 
 
 def test_param_store_layout_cpu():

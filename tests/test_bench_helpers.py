@@ -74,7 +74,7 @@ def test_reference_arm_other_ranks_exit_quietly():
 
 
 def test_committed_bench_line_has_the_contract_keys():
-    line = json.load(open(os.path.join(REPO, "profiles", "r01d_bench_n1.json")))
+    line = json.load(open(os.path.join(REPO, "profiles", "bench_h100_n1.json")))
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
               "vs_baseline", "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
         assert k in line, k

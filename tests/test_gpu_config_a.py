@@ -101,7 +101,7 @@ def test_config_a_full_depth_matches_reference():
     assert e_sum_32 <= 1e-3
     # DPO loss = -logsigmoid(beta * (difference of two log-prob sums of magnitude 700)): a relative tolerance of 1e-3
     # on the sums admits 0.7 absolute on each, i.e. up to beta * 1.4 on the loss, so at 7B depth the loss is
-    # ill-conditioned — the reference's OWN bf16 run moves it by 2.4e-2 relative from its fp32 run, and two B200 builds
+    # ill-conditioned — the reference's OWN bf16 run moves it by 2.4e-2 relative from its fp32 run, and two builds
     # of this repo (different but equally valid summation orders in attention) landed 1.5e-2 and 3.9e-2 from the bf16
     # reference. What CAN be held exactly is consistency: (1) the loss kernel on the CUDA log-probs equals the closed
     # form in fp64 to 1e-5, and (2) the deviation from the reference's loss is bounded by the log-prob deviations that

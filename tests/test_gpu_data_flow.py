@@ -1,5 +1,5 @@
 """-m gpu end-to-end drop-in flow on a synthetic preference dataset: rows without cached log-probs ->
-RLAIFVDataset triggers the frozen-reference pre-pass on the B200 forward kernels -> parquet cache in the
+RLAIFVDataset triggers the frozen-reference pre-pass on the H100 forward kernels -> parquet cache in the
 reference's on-disk format -> DPODataset / DataCollatorForDPODataset -> LLaVA15DPOTrainer.train().
 (muffin/data/datasets.py:27-91, muffin/eval/muffin_inference_logp.py:213-344, muffin/train/train_llava15.py:124-195)"""
 import io

@@ -312,7 +312,6 @@ def test_splice_index_map_and_rows_bit_exact(max_len):
 
 EDGE_FX = os.path.join(os.path.dirname(__file__), "golden_host", "splice_edge_cases.npz")
 # two image tokens in one sequence do not occur on the DPO path (one image per sample); the case is pinned anyway
-# (it passed on B200 in rounds 1 and 2, so it is a plain expectation now)
 EDGE_CASES = ["truncate_max_len_20", "truncate_inside_image", "no_image_sequence", "image_first_and_last", "very_ragged",
               "two_images_one_sequence"]
 

@@ -1,5 +1,5 @@
 """-m gpu: perceiver-resampler piece of BASELINE config (d) (SURVEY.md §8 a13) through the C ABI —
-cross-attention fwd/bwd (tcgen05, shared learned queries), LayerNorm backward, position add, and the whole
+cross-attention fwd/bwd (wgmma, shared learned queries), LayerNorm backward, position add, and the whole
 `Resampler` forward + backward against the oracle that is pinned to the unmodified reference class
 (oracle/gen_golden_resampler.py). Tolerances: bf16 storage vs fp32 oracle => norm-relative errors of ~1e-2."""
 import glob
