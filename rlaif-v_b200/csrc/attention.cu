@@ -677,6 +677,27 @@ static int attention_bwd_impl(const void* q, long long ld_q, const void* k, cons
   B200_REQUIRE(ld_q % 8 == 0 && ld_kv % 8 == 0 && ld_dout % 8 == 0, "attention_bwd: ld must be a multiple of 8");
   B200_REQUIRE(dq ? (ld_dq % 2 == 0 && ((uintptr_t)dq & 3) == 0) : dq_f32 != nullptr, "attention_bwd: dq alignment");
   B200_REQUIRE(ld_dkv % 2 == 0, "attention_bwd: ld_dkv must be even");
+  // attention_delta_kernel reads O and dO rows with 16-byte loads
+  B200_REQUIRE(ld_out % 8 == 0 && ((uintptr_t)out & 15) == 0 && ((uintptr_t)d_out & 15) == 0,
+               "attention_bwd: out / d_out must be 16-byte aligned with ld_out a multiple of 8 (ld_out %lld)", ld_out);
+  const int g = n_heads / n_kv_heads;
+  const int q_nseq = q_shared ? 1 : nseq;
+  int rc;
+  // every tensor map is built (and so validated) before the first launch
+  // dK / dV: K, V resident (128-row boxes), Q / dO streamed in 64-row chunks
+  CUtensorMap tq, tk, tv, tdo;
+  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, q_nseq, Sq, n_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tdo, d_out, ld_dout, nseq, Sq, n_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, 128))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, 128))) return rc;
+  // dQ: Q, dO resident, K / V streamed in 64-row chunks
+  CUtensorMap tq2, tk2, tv2, tdo2;
+  if ((rc = make_qkv_tmap_rows(&tq2, q, ld_q, q_nseq, Sq, n_heads * head_dim, 128))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tdo2, d_out, ld_dout, nseq, Sq, n_heads * head_dim, 128))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tk2, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_qkv_tmap_rows(&tv2, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, BWD_C))) return rc;
+  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dkv_kernel, (int)AttBwdCfg::SMEM_BYTES));
+  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dq_kernel, (int)AttBwdCfg::SMEM_BYTES));
   cudaStream_t st = (cudaStream_t)stream;
   {
     const long long total = (long long)nseq * Sq * n_heads;
@@ -686,32 +707,16 @@ static int attention_bwd_impl(const void* q, long long ld_q, const void* k, cons
                                                         delta_ws, nseq, Sq, n_heads, head_dim);
     B200_CHECK_CUDA(cudaGetLastError());
   }
-  const int g = n_heads / n_kv_heads;
-  const int q_nseq = q_shared ? 1 : nseq;
-  int rc;
-  CUtensorMap tq, tk, tv, tdo;
-  // dK / dV: K, V resident (128-row boxes), Q / dO streamed in 64-row chunks
-  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, q_nseq, Sq, n_heads * head_dim, BWD_C))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tdo, d_out, ld_dout, nseq, Sq, n_heads * head_dim, BWD_C))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, 128))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, 128))) return rc;
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dkv_kernel, (int)AttBwdCfg::SMEM_BYTES));
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_bwd_dq_kernel, (int)AttBwdCfg::SMEM_BYTES));
   {
     dim3 grid((Skv + 127) / 128, n_kv_heads, nseq);
     attention_bwd_dkv_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
         tq, tk, tv, tdo, lse, delta_ws, (bf16*)dk, (bf16*)dv, ld_dkv, Sq, Skv, n_heads, g, causal, q_shared, scale);
     B200_CHECK_CUDA(cudaGetLastError());
   }
-  // dQ: Q, dO resident, K / V streamed in 64-row chunks
-  if ((rc = make_qkv_tmap_rows(&tq, q, ld_q, q_nseq, Sq, n_heads * head_dim, 128))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tdo, d_out, ld_dout, nseq, Sq, n_heads * head_dim, 128))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tk, k, ld_kv, nseq, Skv, n_kv_heads * head_dim, BWD_C))) return rc;
-  if ((rc = make_qkv_tmap_rows(&tv, v, ld_kv, nseq, Skv, n_kv_heads * head_dim, BWD_C))) return rc;
   {
     dim3 grid((Sq + 127) / 128, n_heads, nseq);
     attention_bwd_dq_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
-        tq, tk, tv, tdo, lse, delta_ws, (bf16*)dq, ld_dq, dq_f32, Sq, Skv, n_heads, g, causal, q_shared, scale);
+        tq2, tk2, tv2, tdo2, lse, delta_ws, (bf16*)dq, ld_dq, dq_f32, Sq, Skv, n_heads, g, causal, q_shared, scale);
     B200_CHECK_CUDA(cudaGetLastError());
   }
   return 0;

@@ -410,6 +410,10 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
   B200_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "gemm: lda/ldb must be multiples of 8");
   B200_REQUIRE(!(a_mn_major && !b_mn_major), "gemm: A MN-major with B K-major is not instantiated");
   B200_REQUIRE(((uintptr_t)C & 15) == 0, "gemm: C not 16-byte aligned");
+  // epilogue_pair reads bias and residual as bf16 pairs (32-bit loads at even columns)
+  B200_REQUIRE(!bias || ((uintptr_t)bias & 3) == 0, "gemm: bias not 4-byte aligned");
+  B200_REQUIRE(!residual || (ldr % 2 == 0 && ((uintptr_t)residual & 3) == 0),
+               "gemm: residual must be 4-byte aligned with an even row stride (ldr %lld)", ldr);
   int bn = tile_n;
   if (bn == 0) {
     // the 128 x 256 tile halves the B-operand shared-memory traffic per output element of the 128 x 128 one, and the
