@@ -72,6 +72,9 @@ int rlaifv_gemm_set_tuning(int group_m, int debug);
  * (long-K launches keep the smaller operand's panels resident in the L2); l2 >= 0 forces the given bits together
  * with rlaifv_gemm_set_tuning's group size. Process-wide; results are unaffected. */
 int rlaifv_gemm_set_l2(int l2);
+/* *clusters = the persistent grid's CTA slots for tile_n (128, 256: CTAs; 512: 2-CTA clusters) on the current device:
+ * cudaOccupancyMaxActiveClusters of the kernel, at most num_SMs / cluster size. */
+int rlaifv_gemm_max_active_clusters(int tile_n, int* clusters);
 /* EXPERIMENTAL (default off): run GEMMs with K >= min_k and no bias / activation / residual as n K-slice passes
  * (passes 2.. with C +=) so each pass's operand slabs fit the L2. n <= 1 switches it off. */
 int rlaifv_gemm_set_split_k(int n, int min_k);

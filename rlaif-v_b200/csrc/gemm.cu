@@ -60,6 +60,35 @@ struct GemmCfg {
   static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;  // + barriers + alignment
 };
 
+// Stall accounting, compiled in only with -DRLAIFV_GEMM_STALLS (tools/gemm_step_shapes.py builds that variant; the
+// shipped library has none of it). Every CTA adds its clock64() counts to the device-wide sums below: one math thread
+// per consumer warpgroup times its waits on the `full` barriers and its epilogue, the producer thread its waits on the
+// `empty` barriers. Consumers waiting on `full` = operand supply (L2 / DRAM) is the limit; a producer waiting on
+// `empty` while the consumers do not = the MMA issue rate is; epilogue cycles = tensor-core time lost between tiles.
+enum GemmStall { ST_CTAS, ST_TILES, ST_CONS_TOTAL, ST_CONS_FULL_WAIT, ST_CONS_EPILOGUE, ST_PROD_TOTAL,
+                 ST_PROD_EMPTY_WAIT, ST_FIELDS };
+// The consumers' hooks keep no clock value live across the epilogue or the tile loop (next to the 128 accumulators it
+// would spill, and the counters would then time a different epilogue from the shipped one): a span is added to its
+// sum as -clock64() at its start and +clock64() at its end (stall_mark), a tile's `full` waits are summed in 32 bits,
+// and the consumers' total is the sum of their tiles' spans (first `full` wait to the end of the epilogue).
+#ifdef RLAIFV_GEMM_STALLS
+__device__ unsigned long long g_gemm_stalls[ST_FIELDS];
+__device__ __forceinline__ long long stall_clock() { return clock64(); }
+__device__ __forceinline__ uint32_t stall_clock32() { return (uint32_t)clock(); }
+__device__ __forceinline__ void stall_add(int field, long long v) {
+  atomicAdd(&g_gemm_stalls[field], (unsigned long long)v);
+}
+__device__ __forceinline__ void stall_mark(int field, bool end) {
+  const long long c = clock64();
+  atomicAdd(&g_gemm_stalls[field], (unsigned long long)(end ? c : -c));
+}
+#else
+__device__ __forceinline__ long long stall_clock() { return 0; }
+__device__ __forceinline__ uint32_t stall_clock32() { return 0; }
+__device__ __forceinline__ void stall_add(int, long long) {}
+__device__ __forceinline__ void stall_mark(int, bool) {}
+#endif
+
 __device__ __forceinline__ void tile_coords(int t, int num_m, int num_n, int GROUP_M, int& m_blk, int& n_blk,
                                             bool n_grouped = false) {
   if (n_grouped) {            // same walk with the roles of m and n exchanged: groups of GROUP_M column blocks
@@ -116,11 +145,10 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, long long row,
 // back) the epilogue reads the matching gate / up values and writes d(gate) and d(up) straight into the [M, 2F]
 // gradient of the fused gate|up projection. d is rounded to bf16 first (the reference materialises it); the arithmetic
 // is swiglu_bwd_kernel's (rowops.cu) with an approximate reciprocal (2 ulp, far below the bf16 rounding of the result).
-__device__ __forceinline__ void epilogue_pair_glu(float v0, float v1, long long row, int col, int N,
-                                                  const GemmEpilogue& epi) {
-  const bf16* g_row = epi.glu + row * epi.ld_glu;
-  const float2 g = unpack_bf16(*reinterpret_cast<const uint32_t*>(g_row + col));
-  const float2 u = unpack_bf16(*reinterpret_cast<const uint32_t*>(g_row + N + col));
+// g2 / u2: the bf16 pairs gate[row, col..col+1] and up[row, col..col+1]; c_row: row `row` of C.
+__device__ __forceinline__ void epilogue_pair_glu(float v0, float v1, uint32_t g2, uint32_t u2, bf16* c_row, int col,
+                                                  int N) {
+  const float2 g = unpack_bf16(g2), u = unpack_bf16(u2);
   const float d[2] = {bf16_round(v0), bf16_round(v1)}, gv[2] = {g.x, g.y}, uv[2] = {u.x, u.y};
   float dg[2], du[2];
 #pragma unroll
@@ -129,9 +157,59 @@ __device__ __forceinline__ void epilogue_pair_glu(float v0, float v1, long long 
     du[j] = d[j] * (gv[j] * sg);
     dg[j] = d[j] * uv[j] * (sg * (1.f + gv[j] * (1.f - sg)));
   }
-  bf16* c_row = epi.C + row * epi.ldc;
   *reinterpret_cast<uint32_t*>(c_row + col) = pack_bf16(dg[0], dg[1]);
   *reinterpret_cast<uint32_t*>(c_row + N + col) = pack_bf16(du[0], du[1]);
+}
+
+// Epilogue forms, a template parameter of the kernel so that each launch carries only its own code:
+//   EPI_PLAIN     C = bf16(acc)
+//   EPI_RESIDUAL  C = bf16(bf16(acc) + residual)
+//   EPI_GLU       fused SwiGLU backward (epilogue_pair_glu)
+//   EPI_GENERAL   epilogue_pair: alpha, bias, activation, residual, accumulate in any combination
+// PLAIN and RESIDUAL compute exactly what epilogue_pair computes for those arguments.
+enum EpiKind { EPI_GENERAL, EPI_PLAIN, EPI_RESIDUAL, EPI_GLU };
+
+// One accumulator row of a thread (64 or 128 column pairs, h selects the row of the m64 fragment) in one of the
+// specialised forms. The residual / gate|up values are read CH pairs at a time, all of them before the first store
+// of the group: a store to C may alias them as far as the compiler knows, so loads interleaved with stores would each
+// pay a full global-memory round trip in turn.
+template <int EPI, int BN>
+__device__ __forceinline__ void epilogue_row(const float (&acc)[BN / 2], int h, long long row, int col0, int N,
+                                             const GemmEpilogue& epi) {
+  constexpr int NP = BN / 8;                        // column pairs of this thread per row
+  constexpr int CH = EPI == EPI_GLU ? 16 : NP;      // pairs per load group
+  bf16* c_row = epi.C + row * epi.ldc;
+#pragma unroll
+  for (int i0 = 0; i0 < NP; i0 += CH) {
+    uint32_t x[CH], y[CH];
+#pragma unroll
+    for (int j = 0; j < CH; ++j) {
+      const int col = col0 + (i0 + j) * 8;
+      if constexpr (EPI == EPI_RESIDUAL) {
+        x[j] = col < N ? *reinterpret_cast<const uint32_t*>(epi.residual + row * epi.ldr + col) : 0u;
+      } else if constexpr (EPI == EPI_GLU) {
+        const bf16* g_row = epi.glu + row * epi.ld_glu;
+        x[j] = col < N ? *reinterpret_cast<const uint32_t*>(g_row + col) : 0u;
+        y[j] = col < N ? *reinterpret_cast<const uint32_t*>(g_row + N + col) : 0u;
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < CH; ++j) {
+      const int i = i0 + j, col = col0 + i * 8;
+      if (col >= N) continue;
+      float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+      if constexpr (EPI == EPI_GLU) {
+        epilogue_pair_glu(v0, v1, x[j], y[j], c_row, col, N);
+      } else {
+        if constexpr (EPI == EPI_RESIDUAL) {
+          const float2 q = unpack_bf16(x[j]);
+          v0 = bf16_round(v0) + q.x;
+          v1 = bf16_round(v1) + q.y;
+        }
+        *reinterpret_cast<uint32_t*>(c_row + col) = pack_bf16(v0, v1);
+      }
+    }
+  }
 }
 
 template <bool A_MN, bool B_MN, int BN>
@@ -150,7 +228,7 @@ __device__ __forceinline__ void gemm_mma_stage(float (&acc)[BN / 2], uint32_t a_
 // one 128-row half of B, which TMA multicasts into the shared memory of both CTAs: per output element the pair reads B
 // from L2 once instead of twice. A stage slot is refilled only after the math warps of BOTH CTAs have released it
 // (they arrive on the empty barrier of each CTA), since either producer writes into both.
-template <bool A_MN, bool B_MN, int BN, int CL>
+template <bool A_MN, bool B_MN, int BN, int CL, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -196,6 +274,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       const uint64_t pol_a = l2_policy(epi.l2 & 3), pol_b = l2_policy((epi.l2 >> 2) & 3);
+      const long long clk0 = stall_clock();
+      long long empty_wait = 0;
       int s = 0;
       uint32_t ph = 0;
       for (int t = first_tile; t < num_tiles; t += tile_stride) {
@@ -203,7 +283,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, n_grouped);
         const int m0 = (m_blk * CL + (int)rank) * GEMM_BM, n0 = n_blk * BN;
         for (int kb = 0; kb < num_k; ++kb) {
+          const long long w0 = stall_clock();
           mbar_wait(&empty[s], ph ^ 1);
+          empty_wait += stall_clock() - w0;
           uint8_t* a_dst = smem + s * Cfg::STAGE_BYTES;
           uint8_t* b_dst = a_dst + Cfg::A_BYTES;
           const bool second = kb >= num_k1;
@@ -237,6 +319,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
+      stall_add(ST_CTAS, 1);
+      stall_add(ST_PROD_TOTAL, stall_clock() - clk0);
+      stall_add(ST_PROD_EMPTY_WAIT, empty_wait);
     }
   } else {
     // ------------------------------ MMA + epilogue: 64 rows per warpgroup ------------------------------
@@ -250,12 +335,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       mbar_arrive(&empty[slot]);
       if (CL == 2) mbar_arrive_cluster(&empty[slot], rank ^ 1);
     };
+    const bool timer = (threadIdx.x & 127) == 0;
     for (int t = first_tile; t < num_tiles; t += tile_stride) {
+      if (timer) stall_mark(ST_CONS_TOTAL, false);
       int m_blk, n_blk;
       tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, n_grouped);
       int prev = -1;
+      uint32_t full_wait = 0;
       for (int kb = 0; kb < num_k; ++kb) {
+        full_wait -= stall_clock32();
         mbar_wait(&full[s], ph);
+        full_wait += stall_clock32();
         const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * ATOM_BYTES;   // 64 rows / 2nd M atom
         const uint32_t b_addr = smem_u32(smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES);
         reg_fence(acc);
@@ -271,39 +361,58 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_wait<0>();
       reg_fence(acc);
       if (lane == 0) release(prev);
-      if (epi.debug & 1) continue;
+      if (timer) {
+        stall_add(ST_TILES, 1);
+        stall_add(ST_CONS_FULL_WAIT, full_wait);
+      }
+      if (epi.debug & 1) {
+        if (timer) stall_mark(ST_CONS_TOTAL, true);
+        continue;
+      }
+      if (timer) stall_mark(ST_CONS_EPILOGUE, false);
       const long long row0 = (long long)(m_blk * CL + (int)rank) * GEMM_BM + cw * 64 + (warp & 3) * 16 + g;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long row = row0 + h * 8;
         if (row >= M) continue;
+        if constexpr (EPI != EPI_GENERAL) {
+          epilogue_row<EPI, BN>(acc, h, row, n_blk * BN + tq * 2, N, epi);
+        } else {
 #pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-          const int col = n_blk * BN + i * 8 + tq * 2;
-          if (col >= N) continue;
-          if (epi.glu) epilogue_pair_glu(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], row, col, N, epi);
-          else epilogue_pair(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], row, col, epi);
+          for (int i = 0; i < BN / 8; ++i) {
+            const int col = n_blk * BN + i * 8 + tq * 2;
+            if (col >= N) continue;
+            epilogue_pair(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], row, col, epi);
+          }
         }
+      }
+      if (timer) {
+        stall_mark(ST_CONS_EPILOGUE, true);
+        stall_mark(ST_CONS_TOTAL, true);
       }
     }
   }
   if (CL == 2) cluster_sync_all();    // the peer may still multicast into / arrive on this CTA's shared memory
 }
 
-template <bool A_MN, bool B_MN, int BN, int CL>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2,
-                       const CUtensorMap& tmB2, int M, int N, int K, const GemmSecondSource& src2,
-                       const GemmEpilogue& epi, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<A_MN, B_MN, BN, CL>;
-  B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)Cfg::SMEM_BYTES));
-  const int num_tiles = ((M + CL * GEMM_BM - 1) / (CL * GEMM_BM)) * ((N + BN - 1) / BN);
-  const int slots = num_sms() / CL;
+struct GemmLaunch {
+  CUtensorMap tmA, tmB, tmA2, tmB2;
+  int M, N, K;
+  GemmSecondSource src2;
+  GemmEpilogue epi;
+  cudaStream_t stream;
+};
+
+// CTA slots of the persistent grid: the clusters of CL CTAs (each ~193 KB of shared memory, one per SM) that can be
+// resident at once, asked once per kernel. num_sms() / CL would overstate it when a GPC's free SMs cannot all be
+// paired, and every cluster of the grid beyond the resident ones would start its whole tile range only after another
+// cluster had finished its own.
+template <typename Kern>
+static int resident_clusters(Kern kern, int CL, int smem_bytes) {
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((num_tiles < slots ? num_tiles : slots) * CL);
+  cfg.gridDim = dim3(num_sms() / CL * CL);
   cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = stream;
+  cfg.dynamicSmemBytes = smem_bytes;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = CL;
@@ -311,8 +420,57 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmA2, tmB2, M, N, K, src2, epi));
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, (const void*)kern, &cfg) != cudaSuccess || n <= 0) {
+    cudaGetLastError();
+    n = num_sms() / CL;
+  }
+  return n < num_sms() / CL ? n : num_sms() / CL;
+}
+
+template <bool A_MN, bool B_MN, int BN, int CL, int EPI>
+static int launch_gemm(const GemmLaunch& L) {
+  using Cfg = GemmCfg<BN>;
+  auto kern = gemm_bf16_kernel<A_MN, B_MN, BN, CL, EPI>;
+  B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)Cfg::SMEM_BYTES));
+  static int slots_per_device[64] = {};
+  int dev = 0;
+  B200_CHECK_CUDA(cudaGetDevice(&dev));
+  int& slots = slots_per_device[dev & 63];
+  if (slots == 0) slots = resident_clusters(kern, CL, (int)Cfg::SMEM_BYTES);
+  const int num_tiles = ((L.M + CL * GEMM_BM - 1) / (CL * GEMM_BM)) * ((L.N + BN - 1) / BN);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((num_tiles < slots ? num_tiles : slots) * CL);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+  cfg.stream = L.stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = CL;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, L.tmA, L.tmB, L.tmA2, L.tmB2, L.M, L.N, L.K, L.src2, L.epi));
   return 0;
+}
+
+template <bool A_MN, bool B_MN, int EPI>
+static int launch_tile(int bn, const GemmLaunch& L) {
+  return bn == 512 ? launch_gemm<A_MN, B_MN, 256, 2, EPI>(L)
+       : bn == 256 ? launch_gemm<A_MN, B_MN, 256, 1, EPI>(L)
+                   : launch_gemm<A_MN, B_MN, 128, 1, EPI>(L);
+}
+
+// wgrad (A MN-major) launches have no residual or SwiGLU form: plain or general only.
+template <bool A_MN, bool B_MN>
+static int launch_epi(int kind, int bn, const GemmLaunch& L) {
+  if (kind == EPI_PLAIN) return launch_tile<A_MN, B_MN, EPI_PLAIN>(bn, L);
+  if constexpr (!A_MN) {
+    if (kind == EPI_RESIDUAL) return launch_tile<A_MN, B_MN, EPI_RESIDUAL>(bn, L);
+    if (kind == EPI_GLU) return launch_tile<A_MN, B_MN, EPI_GLU>(bn, L);
+  }
+  return launch_tile<A_MN, B_MN, EPI_GENERAL>(bn, L);
 }
 
 // Build the tensor map of one operand. K-major: tensor [rows][kdim] (ld elements per row),
@@ -335,6 +493,19 @@ static int operand_tmap(CUtensorMap* tm, const void* ptr, long long ld, bool mn_
 }  // namespace b200
 
 using namespace b200;
+
+#ifdef RLAIFV_GEMM_STALLS
+// Stall-accounting build only (not in include/rlaifv_b200.h): copy out / zero the GemmStall sums.
+extern "C" int rlaifv_gemm_stalls_read(unsigned long long* host, int reset) {
+  B200_CHECK_CUDA(cudaDeviceSynchronize());
+  B200_CHECK_CUDA(cudaMemcpyFromSymbol(host, g_gemm_stalls, sizeof(unsigned long long) * ST_FIELDS));
+  if (reset) {
+    const unsigned long long zero[ST_FIELDS] = {};
+    B200_CHECK_CUDA(cudaMemcpyToSymbol(g_gemm_stalls, zero, sizeof(zero)));
+  }
+  return ST_FIELDS;
+}
+#endif
 
 static int g_group_m = 16;
 static int g_debug = 0;
@@ -384,6 +555,8 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
                      int K2 = 0, int r2 = 0, int n_sub = 0, const void* glu = nullptr, long long ld_glu = 0) {
   B200_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
   if (glu) {
+    // the SwiGLU-backward epilogue is instantiated for K-major A only (launch_epi)
+    B200_REQUIRE(!a_mn_major, "gemm (swiglu_bwd epilogue): A must be K-major");
     B200_REQUIRE(!bias && !residual && act == 0 && !accumulate && alpha == 1.0f,
                  "gemm (swiglu_bwd epilogue): no bias / residual / activation / accumulate / alpha");
     B200_REQUIRE(N % 64 == 0 && ld_glu % 8 == 0 && ld_glu >= 2LL * N && ldc >= 2LL * N,
@@ -450,7 +623,16 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
     rc = operand_tmap(&tmB2, B2, ldb2, b_mn_major != 0, N, K2, bn == 512 ? 128 : bn);
     if (rc) return rc;
   }
-  GemmEpilogue epi;
+  GemmLaunch L;
+  L.tmA = tmA;
+  L.tmB = tmB;
+  L.tmA2 = tmA2;
+  L.tmB2 = tmB2;
+  L.M = M;
+  L.N = N;
+  L.K = K;
+  L.src2 = src2;
+  GemmEpilogue& epi = L.epi;
   epi.C = (bf16*)C;
   epi.ldc = ldc;
   epi.bias = (const bf16*)bias;
@@ -466,18 +648,33 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
   epi.l2 = 0;
   if (g_l2 < 0) l2_auto_policy(M, N, K, &epi.l2, &epi.group_m);
   else epi.l2 = g_l2 & 0x4f;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (!a_mn_major && !b_mn_major)
-    return bn == 512 ? launch_gemm<false, false, 256, 2>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
-         : bn == 256 ? launch_gemm<false, false, 256, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
-                     : launch_gemm<false, false, 128, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st);
-  if (!a_mn_major && b_mn_major)
-    return bn == 512 ? launch_gemm<false, true, 256, 2>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
-         : bn == 256 ? launch_gemm<false, true, 256, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
-                     : launch_gemm<false, true, 128, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st);
-  return bn == 512 ? launch_gemm<true, true, 256, 2>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
-       : bn == 256 ? launch_gemm<true, true, 256, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st)
-                   : launch_gemm<true, true, 128, 1>(tmA, tmB, tmA2, tmB2, M, N, K, src2, epi, st);
+  L.stream = (cudaStream_t)stream;
+  const bool plain = !bias && act == 0 && !accumulate && alpha == 1.0f;
+  const int kind = glu ? EPI_GLU : !plain ? EPI_GENERAL : residual ? EPI_RESIDUAL : EPI_PLAIN;
+  if (!a_mn_major && !b_mn_major) return launch_epi<false, false>(kind, bn, L);
+  if (!a_mn_major && b_mn_major) return launch_epi<false, true>(kind, bn, L);
+  return launch_epi<true, true>(kind, bn, L);
+}
+
+extern "C" int rlaifv_gemm_max_active_clusters(int tile_n, int* clusters) {
+  B200_REQUIRE(tile_n == 128 || tile_n == 256 || tile_n == 512, "gemm: tile_n must be 128, 256 or 512");
+  B200_REQUIRE(clusters, "gemm_max_active_clusters: null output");
+  const int cl = tile_n == 512 ? 2 : 1, bn = tile_n == 512 ? 256 : tile_n;
+  const int smem = bn == 256 ? (int)GemmCfg<256>::SMEM_BYTES : (int)GemmCfg<128>::SMEM_BYTES;
+  if (tile_n == 512) {
+    auto k = gemm_bf16_kernel<false, false, 256, 2, EPI_PLAIN>;
+    B200_CHECK_CUDA(configure_smem_once((const void*)k, smem));
+    *clusters = resident_clusters(k, cl, smem);
+  } else if (bn == 256) {
+    auto k = gemm_bf16_kernel<false, false, 256, 1, EPI_PLAIN>;
+    B200_CHECK_CUDA(configure_smem_once((const void*)k, smem));
+    *clusters = resident_clusters(k, cl, smem);
+  } else {
+    auto k = gemm_bf16_kernel<false, false, 128, 1, EPI_PLAIN>;
+    B200_CHECK_CUDA(configure_smem_once((const void*)k, smem));
+    *clusters = resident_clusters(k, cl, smem);
+  }
+  return 0;
 }
 
 extern "C" int rlaifv_gemm_bf16(const void* A, long long lda, int a_mn_major, const void* B, long long ldb,

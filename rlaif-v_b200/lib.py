@@ -33,6 +33,7 @@ _SIGNATURES = {
                                    c_int, c_int, c_float, c_void_p],
     "rlaifv_gemm_set_tuning": [c_int, c_int],
     "rlaifv_gemm_set_l2": [c_int],
+    "rlaifv_gemm_max_active_clusters": [c_int, c_void_p],
     "rlaifv_gemm_set_split_k": [c_int, c_int],
     "rlaifv_rmsnorm_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p],
     "rlaifv_rmsnorm_bwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
