@@ -63,8 +63,14 @@ int rlaifv_gemm_bf16_swiglu_bwd(const void* A, long long lda, const void* B, lon
                                 const void* A2, long long lda2, const void* B2, long long ldb2, int K2, const void* gu,
                                 long long ld_gu, void* dgu, long long ld_dgu, int M, int F, int K, void* stream);
 
-/* raster group size (row-blocks per group, default 16) and a profiling switch (debug: bit0 skip the stores of C —
- * results are then garbage; for roofline experiments only). */
+/* raster group size (row-blocks per group, 0 keeps the current one; default 16) and debug switches:
+ *   bit 0: skip the epilogue, stores of C included (mainloop only; results are then garbage; for roofline
+ *          experiments only);
+ *   bit 1: run the plain, residual and SwiGLU-backward forms with the register epilogue (each thread stores C straight
+ *          from its accumulators) instead of the staged one (C through shared memory and TMA stores). Results are
+ *          bit-identical; for A/B tests and timings. The register epilogue also runs every launch with bias, activation,
+ *          alpha or accumulate, and a residual that is not 16-byte aligned or whose row stride is not a multiple of 8.
+ * Process-wide. */
 int rlaifv_gemm_set_tuning(int group_m, int debug);
 /* L2 policy of the GEMM's TMA operand loads: bits 0-1 A loads, 2-3 B loads (0 normal, 1 evict first, 2 evict last;
  * bits 4-5 are accepted and ignored); bit 6: raster walks n-fastest inside groups of group_m column blocks instead of m-fastest

@@ -1,7 +1,8 @@
 // bf16 x bf16 -> fp32 -> bf16 GEMM for sm_90a: TMA-staged SWIZZLE_128B shared-memory tiles feeding wgmma.mma_async
 // (64 x BN x 16 per warpgroup), persistent warp-specialised CTAs: one producer warpgroup issues the TMA loads of a
-// multi-stage ring, two math warpgroups each own 64 rows of the 128 x BN tile and run the epilogue straight from their
-// accumulator registers while the producer already streams the next tile's operands.
+// multi-stage ring, two math warpgroups each own 64 rows of the 128 x BN tile and run the epilogue while the producer
+// already streams the next tile's operands. The plain, residual and SwiGLU-backward epilogues write C through shared
+// memory with TMA stores (epilogue_staged); the general one stores from the accumulator registers.
 //
 // One kernel covers the three operand forms a linear layer needs (reference call sites: every
 // nn.Linear inside HF LlamaDecoderLayer / CLIPEncoderLayer / mm_projector —
@@ -28,7 +29,7 @@ struct GemmEpilogue {
   int act;         // 0 none, 1 GELU(erf), 2 quick_gelu (x*sigmoid(1.702x))
   int accumulate;  // C = C + result (fp32 add of the old bf16 value)
   int group_m;     // raster: tiles are walked m-fastest inside groups of `group_m` row-blocks
-  int debug;       // profiling only: bit0 skip global stores
+  int debug;       // profiling only: bit0 skip the epilogue (mainloop only)
   float alpha;     // != 1: result = bf16(bf16(acc) * alpha) first (LoRA scaling, peft: lora_B(...) * scaling)
   const bf16* glu; // non-null: fused SwiGLU backward. The accumulator tile is d(act) [M, N = F]; glu = [gate | up] rows
   long long ld_glu;//   [M, 2F]; C = d[gate | up] [M, 2F]: C[:, n] = d*u*silu'(g), C[:, F + n] = d*silu(g)  (d = bf16(acc))
@@ -51,13 +52,32 @@ constexpr int GEMM_BK = 64;
 constexpr int GEMM_THREADS = 384;
 constexpr uint32_t ATOM_BYTES = 64 * 128;   // one [64 rows][64 bf16] SWIZZLE_128B atom
 
-template <int BN>
+// Epilogue forms, a template parameter of the kernel so that each launch carries only its own code:
+//   EPI_PLAIN     C = bf16(acc)
+//   EPI_RESIDUAL  C = bf16(bf16(acc) + residual)
+//   EPI_GLU       fused SwiGLU backward (epilogue_pair_glu)
+//   EPI_GENERAL   epilogue_pair: alpha, bias, activation, residual, accumulate in any combination
+// PLAIN and RESIDUAL compute exactly what epilogue_pair computes for those arguments.
+enum EpiKind { EPI_GENERAL, EPI_PLAIN, EPI_RESIDUAL, EPI_GLU };
+
+// STAGED: the plain, residual and SwiGLU forms write C through SWIZZLE_128B staging atoms in the 32 KB of shared memory
+// the ring leaves free (TMA stores; the residual and gate|up come in by TMA loads into the same atoms). Each math
+// warpgroup owns two atoms: SLOTS staging slots of SLOT_ATOMS atoms, one subtile of 64 rows x 64 columns (SwiGLU: its
+// gate and up halves) per slot. The SwiGLU form is thus single-buffered. A double-buffered one (a ring of 3 stages at
+// tile 256, 5 at tile 128, to free the atoms) was 6 % slower on the LoRA step's down-projection dgrad (H100 SXM, 400 W):
+// that launch waits on operand supply more than on its epilogue.
+template <int BN, int EPI = EPI_GENERAL, bool STAGED = false>
 struct GemmCfg {
   static constexpr int STAGES = (BN == 256) ? 4 : 6;    // 192 KB of the 227 KB a block may use
   static constexpr uint32_t A_BYTES = GEMM_BM * GEMM_BK * 2;
   static constexpr uint32_t B_BYTES = BN * GEMM_BK * 2;
   static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;  // + barriers + alignment
+  static constexpr int SLOT_ATOMS = EPI == EPI_GLU ? 2 : 1;
+  static constexpr int SLOTS = EPI == EPI_GLU ? 1 : 2;
+  static constexpr uint32_t WG_STAGING_BYTES = STAGED ? SLOTS * SLOT_ATOMS * ATOM_BYTES : 0;
+  static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 2 * WG_STAGING_BYTES + 256 + 1024;  // + barriers
+                                                                                                   //   + alignment
+  static_assert(SMEM_BYTES <= 232448, "over the 227 KB of shared memory a block may opt in to");
 };
 
 // Stall accounting, compiled in only with -DRLAIFV_GEMM_STALLS (tools/gemm_step_shapes.py builds that variant; the
@@ -146,8 +166,9 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, long long row,
 // gradient of the fused gate|up projection. d is rounded to bf16 first (the reference materialises it); the arithmetic
 // is swiglu_bwd_kernel's (rowops.cu) with an approximate reciprocal (2 ulp, far below the bf16 rounding of the result).
 // g2 / u2: the bf16 pairs gate[row, col..col+1] and up[row, col..col+1]; c_row: row `row` of C.
-__device__ __forceinline__ void epilogue_pair_glu(float v0, float v1, uint32_t g2, uint32_t u2, bf16* c_row, int col,
-                                                  int N) {
+// swiglu_bwd_pair returns the packed pairs d[gate] (dg2) and d[up] (du2).
+__device__ __forceinline__ void swiglu_bwd_pair(float v0, float v1, uint32_t g2, uint32_t u2, uint32_t& dg2,
+                                                uint32_t& du2) {
   const float2 g = unpack_bf16(g2), u = unpack_bf16(u2);
   const float d[2] = {bf16_round(v0), bf16_round(v1)}, gv[2] = {g.x, g.y}, uv[2] = {u.x, u.y};
   float dg[2], du[2];
@@ -157,17 +178,16 @@ __device__ __forceinline__ void epilogue_pair_glu(float v0, float v1, uint32_t g
     du[j] = d[j] * (gv[j] * sg);
     dg[j] = d[j] * uv[j] * (sg * (1.f + gv[j] * (1.f - sg)));
   }
-  *reinterpret_cast<uint32_t*>(c_row + col) = pack_bf16(dg[0], dg[1]);
-  *reinterpret_cast<uint32_t*>(c_row + N + col) = pack_bf16(du[0], du[1]);
+  dg2 = pack_bf16(dg[0], dg[1]);
+  du2 = pack_bf16(du[0], du[1]);
 }
-
-// Epilogue forms, a template parameter of the kernel so that each launch carries only its own code:
-//   EPI_PLAIN     C = bf16(acc)
-//   EPI_RESIDUAL  C = bf16(bf16(acc) + residual)
-//   EPI_GLU       fused SwiGLU backward (epilogue_pair_glu)
-//   EPI_GENERAL   epilogue_pair: alpha, bias, activation, residual, accumulate in any combination
-// PLAIN and RESIDUAL compute exactly what epilogue_pair computes for those arguments.
-enum EpiKind { EPI_GENERAL, EPI_PLAIN, EPI_RESIDUAL, EPI_GLU };
+__device__ __forceinline__ void epilogue_pair_glu(float v0, float v1, uint32_t g2, uint32_t u2, bf16* c_row, int col,
+                                                  int N) {
+  uint32_t dg2, du2;
+  swiglu_bwd_pair(v0, v1, g2, u2, dg2, du2);
+  *reinterpret_cast<uint32_t*>(c_row + col) = dg2;
+  *reinterpret_cast<uint32_t*>(c_row + N + col) = du2;
+}
 
 // One accumulator row of a thread (64 or 128 column pairs, h selects the row of the m64 fragment) in one of the
 // specialised forms. The residual / gate|up values are read CH pairs at a time, all of them before the first store
@@ -212,6 +232,131 @@ __device__ __forceinline__ void epilogue_row(const float (&acc)[BN / 2], int h, 
   }
 }
 
+// Staged epilogue (STAGED kernels) of one math warpgroup's 64 rows x BN columns, one 64 x 64 subtile per staging slot,
+// slots taken round robin. Per subtile:
+//   1. the slot is free. Plain: the elected thread waits until the bulk store that last used it has been read out,
+//      then a named barrier (the warpgroup's 128 threads). Residual / SwiGLU: every thread waits on the slot's
+//      mbarrier for the TMA load of this subtile's operands, which was issued only after the slot's previous store had
+//      been read out;
+//   2. every thread writes its accumulator fragment with stmatrix at the swizzled addresses (residual / SwiGLU: in
+//      place, after reading its operand pairs there with ldmatrix; each warp reads and writes only its own 16 rows);
+//   3. fence.proxy.async, named barrier, and the elected thread issues the TMA store(s) as one bulk group. It then
+//      refills the slot with the operands of subtile j + SLOTS once the store has read it out.
+// No one waits for the stores at the end of a tile: the next tile's MMAs run while the copy engine drains the slots.
+// TMA clips the boxes at M and N, so M tails and the neighbouring columns of column-block views stay untouched, and a
+// C that aliases the residual is read before it is written (a subtile's load lands before its store is issued). The
+// values and rounding points are epilogue_row's.
+// Shared-window addresses (32 bits: they stay live across the mainloop, next to the accumulators).
+struct StagedEpi {
+  uint32_t slots;   // this warpgroup's staging atoms
+  uint32_t bar;     // one mbarrier per slot: TMA loads of the residual / gate|up subtiles
+  int row0;         // first of the warpgroup's 64 rows
+  int n0;           // first column of the tile (SwiGLU: in d(act), i.e. in the gate half)
+  // subtiles inside N; 0 when all of the warpgroup's rows are past M (recomputed where needed: M and N are kernel
+  // parameters, a register held across the mainloop is not)
+  __device__ __forceinline__ int nsub(int M, int N, int BN) const {
+    return row0 < M ? min(BN / 64, (N - n0 + 63) / 64) : 0;
+  }
+};
+
+// TMA load of subtile j's residual (or gate and up) into its slot; elected thread only.
+template <int EPI, typename Cfg>
+__device__ __forceinline__ void staged_load(const StagedEpi& se, int j, const CUtensorMap* tmR, int N) {
+  const int slot = j % Cfg::SLOTS;
+  uint8_t* dst = smem_ptr<uint8_t>(se.slots + slot * Cfg::SLOT_ATOMS * ATOM_BYTES);
+  uint64_t* bar = smem_ptr<uint64_t>(se.bar + slot * 8);
+  mbar_arrive_expect_tx(bar, Cfg::SLOT_ATOMS * ATOM_BYTES);
+  tma_load_2d(dst, tmR, bar, se.n0 + 64 * j, se.row0);
+  if constexpr (EPI == EPI_GLU) tma_load_2d(dst + ATOM_BYTES, tmR, bar, N + se.n0 + 64 * j, se.row0);
+}
+
+// Elected thread, as the tile's mainloop starts (the loads land while its MMAs run): the first SLOTS subtiles'
+// operands, once the previous tile's stores have been read out of the slots.
+template <int EPI, int BN, typename Cfg>
+__device__ __forceinline__ void staged_prefetch(const StagedEpi& se, const CUtensorMap* tmR, int M, int N) {
+  tma_store_wait_read<0>();
+  const int nsub = se.nsub(M, N, BN);
+  for (int j = 0; j < Cfg::SLOTS && j < nsub; ++j) staged_load<EPI, Cfg>(se, j, tmR, N);
+}
+
+// phase: bit 1 + slot is the parity of the slot's mbarrier (bit 0 belongs to the caller).
+template <int EPI, int BN, typename Cfg>
+__device__ __forceinline__ void epilogue_staged(const float (&acc)[BN / 2], const StagedEpi& se, uint32_t& phase,
+                                                const CUtensorMap* tmC, const CUtensorMap* tmR, int M, int N,
+                                                bool leader, int bar_id) {
+  const int nsub = se.nsub(M, N, BN);
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  // stmatrix / ldmatrix x4 over column pairs (i, i + 1), i = 8j + 2p: matrix q is pair i + (q >> 1), row half q & 1;
+  // this lane addresses row r of matrix q
+  const int q = lane >> 3, r = lane & 7;
+  const uint32_t row_addr = se.slots + (16 * w + 8 * (q & 1) + r) * 128;
+#pragma unroll
+  for (int j = 0; j < BN / 64; ++j) {
+    if (j >= nsub) break;
+    const int slot = j % Cfg::SLOTS;
+    const uint32_t slot_off = slot * Cfg::SLOT_ATOMS * ATOM_BYTES;
+    if constexpr (EPI == EPI_PLAIN) {
+      if (leader) {
+        if (j == 0) tma_store_wait_read<0>();   // the previous tile's stores: long done
+        else tma_store_wait_read<1>();          // subtile j - 2's store, which used this slot
+      }
+      named_bar_sync(bar_id, 128);
+    } else {
+      mbar_wait(smem_ptr<uint64_t>(se.bar + slot * 8), (phase >> (1 + slot)) & 1);
+      phase ^= 2u << slot;
+    }
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      if constexpr (EPI == EPI_GLU) {
+        // x2 halves (pair i, both row halves): gate and up in place, four registers fewer live than x4
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const uint32_t addr = row_addr + slot_off + (((2 * p + hf) ^ r) << 4);
+          const int i = 8 * j + 2 * p + hf;
+          uint32_t x[2], y[2];
+          ldmatrix_x2(addr, x);
+          ldmatrix_x2(addr + ATOM_BYTES, y);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) swiglu_bwd_pair(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], x[h], y[h], x[h], y[h]);
+          stmatrix_x2(addr, x);
+          stmatrix_x2(addr + ATOM_BYTES, y);
+        }
+      } else {
+        const uint32_t addr = row_addr + slot_off + (((2 * p + (q >> 1)) ^ r) << 4);   // SWIZZLE_128B: chunk ^ row % 8
+        uint32_t x[4];   // residual pairs, then (in place) the results
+        if constexpr (EPI == EPI_RESIDUAL) ldmatrix_x4(addr, x);
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          const int i = 8 * j + 2 * p + (m >> 1), h = m & 1;
+          float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+          if constexpr (EPI == EPI_RESIDUAL) {
+            const float2 rv = unpack_bf16(x[m]);
+            v0 = bf16_round(v0) + rv.x;
+            v1 = bf16_round(v1) + rv.y;
+          }
+          x[m] = pack_bf16(v0, v1);
+        }
+        stmatrix_x4(addr, x);
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(bar_id, 128);
+    if (leader) {
+      const uint8_t* src = smem_ptr<uint8_t>(se.slots + slot_off);
+      const int col = se.n0 + 64 * j;
+      tma_store_2d(tmC, src, col, se.row0);
+      if constexpr (EPI == EPI_GLU) tma_store_2d(tmC, src + ATOM_BYTES, N + col, se.row0);
+      tma_store_commit();
+      if constexpr (EPI != EPI_PLAIN) {
+        if (j + Cfg::SLOTS < nsub) {
+          tma_store_wait_read<0>();
+          staged_load<EPI, Cfg>(se, j + Cfg::SLOTS, tmR, N);
+        }
+      }
+    }
+  }
+}
+
 template <bool A_MN, bool B_MN, int BN>
 __device__ __forceinline__ void gemm_mma_stage(float (&acc)[BN / 2], uint32_t a_addr, uint32_t b_addr, int first) {
 #pragma unroll
@@ -228,18 +373,22 @@ __device__ __forceinline__ void gemm_mma_stage(float (&acc)[BN / 2], uint32_t a_
 // one 128-row half of B, which TMA multicasts into the shared memory of both CTAs: per output element the pair reads B
 // from L2 once instead of twice. A stage slot is refilled only after the math warps of BOTH CTAs have released it
 // (they arrive on the empty barrier of each CTA), since either producer writes into both.
-template <bool A_MN, bool B_MN, int BN, int CL, int EPI>
+// tmC / tmR (STAGED only): C as {N, M} (SwiGLU: {2F, M}) and the residual (SwiGLU: gate|up) in 64 x 64 boxes.
+template <bool A_MN, bool B_MN, int BN, int CL, int EPI, bool STAGED>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
                  int M, int N, int K, GemmSecondSource src2, GemmEpilogue epi) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, EPI, STAGED>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;     // 2 x WG_STAGING_BYTES, 1024-byte aligned
+  uint64_t* full = reinterpret_cast<uint64_t*>(staging + 2 * Cfg::WG_STAGING_BYTES);
   uint64_t* empty = full + STAGES;
+  uint64_t* ebar = empty + STAGES;                          // STAGED: SLOTS per math warpgroup
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -264,6 +413,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 8 * CL);     // lane 0 of each of the 8 math warps (of both CTAs of a pair)
     }
+    if (STAGED)
+      for (int i = 0; i < 2 * Cfg::SLOTS; ++i) mbar_init(&ebar[i], 1);
     fence_barrier_init();
   }
   if (CL == 2) cluster_sync_all();    // the peer's multicasts and arrives need this CTA's initialised barriers
@@ -330,21 +481,31 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int g = lane >> 2, tq = lane & 3;
     float acc[BN / 2];
     int s = 0;
-    uint32_t ph = 0;
+    uint32_t ph = 0;             // bit 0: parity of the ring's `full` barriers; STAGED: bits 1.. those of the slots
     auto release = [&](int slot) {
       mbar_arrive(&empty[slot]);
       if (CL == 2) mbar_arrive_cluster(&empty[slot], rank ^ 1);
     };
-    const bool timer = (threadIdx.x & 127) == 0;
+    const bool timer = (threadIdx.x & 127) == 0;   // also the warpgroup's elected thread of the staged epilogue
+    StagedEpi se;
+    se.slots = smem_u32(staging + cw * Cfg::WG_STAGING_BYTES);
+    se.bar = smem_u32(ebar + cw * Cfg::SLOTS);
     for (int t = first_tile; t < num_tiles; t += tile_stride) {
       if (timer) stall_mark(ST_CONS_TOTAL, false);
       int m_blk, n_blk;
       tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, n_grouped);
+      if constexpr (STAGED) {
+        se.row0 = (m_blk * CL + (int)rank) * GEMM_BM + cw * 64;
+        se.n0 = n_blk * BN;
+        if constexpr (EPI != EPI_PLAIN) {
+          if (timer && !(epi.debug & 1)) staged_prefetch<EPI, BN, Cfg>(se, &tmR, M, N);
+        }
+      }
       int prev = -1;
       uint32_t full_wait = 0;
       for (int kb = 0; kb < num_k; ++kb) {
         full_wait -= stall_clock32();
-        mbar_wait(&full[s], ph);
+        mbar_wait(&full[s], ph & 1);
         full_wait += stall_clock32();
         const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * ATOM_BYTES;   // 64 rows / 2nd M atom
         const uint32_t b_addr = smem_u32(smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES);
@@ -370,19 +531,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         continue;
       }
       if (timer) stall_mark(ST_CONS_EPILOGUE, false);
-      const long long row0 = (long long)(m_blk * CL + (int)rank) * GEMM_BM + cw * 64 + (warp & 3) * 16 + g;
+      if constexpr (STAGED) {
+        epilogue_staged<EPI, BN, Cfg>(acc, se, ph, &tmC, &tmR, M, N, timer, 1 + cw);
+      } else {
+        const long long row0 = (long long)(m_blk * CL + (int)rank) * GEMM_BM + cw * 64 + (warp & 3) * 16 + g;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const long long row = row0 + h * 8;
-        if (row >= M) continue;
-        if constexpr (EPI != EPI_GENERAL) {
-          epilogue_row<EPI, BN>(acc, h, row, n_blk * BN + tq * 2, N, epi);
-        } else {
+        for (int h = 0; h < 2; ++h) {
+          const long long row = row0 + h * 8;
+          if (row >= M) continue;
+          if constexpr (EPI != EPI_GENERAL) {
+            epilogue_row<EPI, BN>(acc, h, row, n_blk * BN + tq * 2, N, epi);
+          } else {
 #pragma unroll
-          for (int i = 0; i < BN / 8; ++i) {
-            const int col = n_blk * BN + i * 8 + tq * 2;
-            if (col >= N) continue;
-            epilogue_pair(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], row, col, epi);
+            for (int i = 0; i < BN / 8; ++i) {
+              const int col = n_blk * BN + i * 8 + tq * 2;
+              if (col >= N) continue;
+              epilogue_pair(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], row, col, epi);
+            }
           }
         }
       }
@@ -391,12 +556,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         stall_mark(ST_CONS_TOTAL, true);
       }
     }
+    if (STAGED && timer) tma_store_wait_all<0>();   // the slots must outlive the bulk stores that read them
   }
   if (CL == 2) cluster_sync_all();    // the peer may still multicast into / arrive on this CTA's shared memory
 }
 
 struct GemmLaunch {
-  CUtensorMap tmA, tmB, tmA2, tmB2;
+  CUtensorMap tmA, tmB, tmA2, tmB2, tmC, tmR;
   int M, N, K;
   GemmSecondSource src2;
   GemmEpilogue epi;
@@ -428,10 +594,10 @@ static int resident_clusters(Kern kern, int CL, int smem_bytes) {
   return n < num_sms() / CL ? n : num_sms() / CL;
 }
 
-template <bool A_MN, bool B_MN, int BN, int CL, int EPI>
+template <bool A_MN, bool B_MN, int BN, int CL, int EPI, bool STAGED>
 static int launch_gemm(const GemmLaunch& L) {
-  using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<A_MN, B_MN, BN, CL, EPI>;
+  using Cfg = GemmCfg<BN, EPI, STAGED>;
+  auto kern = gemm_bf16_kernel<A_MN, B_MN, BN, CL, EPI, STAGED>;
   B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)Cfg::SMEM_BYTES));
   static int slots_per_device[64] = {};
   int dev = 0;
@@ -451,26 +617,32 @@ static int launch_gemm(const GemmLaunch& L) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, L.tmA, L.tmB, L.tmA2, L.tmB2, L.M, L.N, L.K, L.src2, L.epi));
+  B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, L.tmA, L.tmB, L.tmA2, L.tmB2, L.tmC, L.tmR, L.M, L.N, L.K, L.src2,
+                                     L.epi));
   return 0;
 }
 
-template <bool A_MN, bool B_MN, int EPI>
+template <bool A_MN, bool B_MN, int EPI, bool STAGED>
 static int launch_tile(int bn, const GemmLaunch& L) {
-  return bn == 512 ? launch_gemm<A_MN, B_MN, 256, 2, EPI>(L)
-       : bn == 256 ? launch_gemm<A_MN, B_MN, 256, 1, EPI>(L)
-                   : launch_gemm<A_MN, B_MN, 128, 1, EPI>(L);
+  return bn == 512 ? launch_gemm<A_MN, B_MN, 256, 2, EPI, STAGED>(L)
+       : bn == 256 ? launch_gemm<A_MN, B_MN, 256, 1, EPI, STAGED>(L)
+                   : launch_gemm<A_MN, B_MN, 128, 1, EPI, STAGED>(L);
 }
 
-// wgrad (A MN-major) launches have no residual or SwiGLU form: plain or general only.
+// wgrad (A MN-major) launches have no residual or SwiGLU form: plain or general only. The general form has no staged
+// kernel; the other forms have both, the register epilogue kept for the launches the staged one cannot take (gemm_impl).
 template <bool A_MN, bool B_MN>
-static int launch_epi(int kind, int bn, const GemmLaunch& L) {
-  if (kind == EPI_PLAIN) return launch_tile<A_MN, B_MN, EPI_PLAIN>(bn, L);
+static int launch_epi(int kind, bool staged, int bn, const GemmLaunch& L) {
+  if (kind == EPI_PLAIN)
+    return staged ? launch_tile<A_MN, B_MN, EPI_PLAIN, true>(bn, L) : launch_tile<A_MN, B_MN, EPI_PLAIN, false>(bn, L);
   if constexpr (!A_MN) {
-    if (kind == EPI_RESIDUAL) return launch_tile<A_MN, B_MN, EPI_RESIDUAL>(bn, L);
-    if (kind == EPI_GLU) return launch_tile<A_MN, B_MN, EPI_GLU>(bn, L);
+    if (kind == EPI_RESIDUAL)
+      return staged ? launch_tile<A_MN, B_MN, EPI_RESIDUAL, true>(bn, L)
+                    : launch_tile<A_MN, B_MN, EPI_RESIDUAL, false>(bn, L);
+    if (kind == EPI_GLU)
+      return staged ? launch_tile<A_MN, B_MN, EPI_GLU, true>(bn, L) : launch_tile<A_MN, B_MN, EPI_GLU, false>(bn, L);
   }
-  return launch_tile<A_MN, B_MN, EPI_GENERAL>(bn, L);
+  return launch_tile<A_MN, B_MN, EPI_GENERAL, false>(bn, L);
 }
 
 // Build the tensor map of one operand. K-major: tensor [rows][kdim] (ld elements per row),
@@ -508,14 +680,14 @@ extern "C" int rlaifv_gemm_stalls_read(unsigned long long* host, int reset) {
 #endif
 
 static int g_group_m = 16;
-static int g_debug = 0;
+static int g_debug = 0;     // bit 0: GemmEpilogue::debug; bit 1: register epilogue for every form (gemm_impl)
 extern "C" int rlaifv_gemm_set_tuning(int group_m, int debug) {
   if (group_m > 0) g_group_m = group_m;
-  g_debug = debug & 1;
+  g_debug = debug & 3;
   return 0;
 }
 // L2 policy of the operand loads and the tile raster (GemmEpilogue::l2; bits 4-5, the C-store hint, are accepted and
-// ignored: C leaves through ordinary stores). l2 < 0 (default): chosen per launch by l2_auto_policy() below; l2 >= 0:
+// ignored: C leaves through plain TMA stores or ordinary stores). l2 < 0 (default): chosen per launch by l2_auto_policy() below; l2 >= 0:
 // the given bits for every launch.
 static int g_l2 = -1;
 extern "C" int rlaifv_gemm_set_l2(int l2) {
@@ -628,6 +800,28 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
   L.tmB = tmB;
   L.tmA2 = tmA2;
   L.tmB2 = tmB2;
+  const bool plain = !bias && act == 0 && !accumulate && alpha == 1.0f;
+  const int kind = glu ? EPI_GLU : !plain ? EPI_GENERAL : residual ? EPI_RESIDUAL : EPI_PLAIN;
+  // The staged epilogue moves C, the residual and gate|up in 64 x 64 TMA boxes: a residual needs the 16-byte alignment
+  // of a tensor map (C and gate|up are required to have it above).
+  const bool staged = kind != EPI_GENERAL && !(g_debug & 2) &&
+                      (kind != EPI_RESIDUAL || (((uintptr_t)residual & 15) == 0 && ldr % 8 == 0));
+  if (staged) {
+    // {columns, rows} with the real row strides: TMA clips every box at N (2F) and M
+    const uint32_t box[2] = {64, 64};
+    const uint64_t c_dims[2] = {(uint64_t)(glu ? 2LL * N : N), (uint64_t)M}, c_str[1] = {(uint64_t)ldc * 2};
+    rc = make_tmap_bf16(&L.tmC, C, 2, c_dims, c_str, box);
+    if (rc) return rc;
+    L.tmR = L.tmC;
+    if (kind != EPI_PLAIN) {
+      const uint64_t r_dims[2] = {(uint64_t)(glu ? 2LL * N : N), (uint64_t)M};
+      const uint64_t r_str[1] = {(uint64_t)(glu ? ld_glu : ldr) * 2};
+      rc = make_tmap_bf16(&L.tmR, glu ? glu : residual, 2, r_dims, r_str, box);
+      if (rc) return rc;
+    }
+  } else {
+    L.tmC = L.tmR = tmA;     // not read by the register epilogue
+  }
   L.M = M;
   L.N = N;
   L.K = K;
@@ -649,28 +843,28 @@ static int gemm_impl(const void* A, long long lda, int a_mn_major, const void* B
   if (g_l2 < 0) l2_auto_policy(M, N, K, &epi.l2, &epi.group_m);
   else epi.l2 = g_l2 & 0x4f;
   L.stream = (cudaStream_t)stream;
-  const bool plain = !bias && act == 0 && !accumulate && alpha == 1.0f;
-  const int kind = glu ? EPI_GLU : !plain ? EPI_GENERAL : residual ? EPI_RESIDUAL : EPI_PLAIN;
-  if (!a_mn_major && !b_mn_major) return launch_epi<false, false>(kind, bn, L);
-  if (!a_mn_major && b_mn_major) return launch_epi<false, true>(kind, bn, L);
-  return launch_epi<true, true>(kind, bn, L);
+  if (!a_mn_major && !b_mn_major) return launch_epi<false, false>(kind, staged, bn, L);
+  if (!a_mn_major && b_mn_major) return launch_epi<false, true>(kind, staged, bn, L);
+  return launch_epi<true, true>(kind, staged, bn, L);
 }
 
 extern "C" int rlaifv_gemm_max_active_clusters(int tile_n, int* clusters) {
   B200_REQUIRE(tile_n == 128 || tile_n == 256 || tile_n == 512, "gemm: tile_n must be 128, 256 or 512");
   B200_REQUIRE(clusters, "gemm_max_active_clusters: null output");
   const int cl = tile_n == 512 ? 2 : 1, bn = tile_n == 512 ? 256 : tile_n;
-  const int smem = bn == 256 ? (int)GemmCfg<256>::SMEM_BYTES : (int)GemmCfg<128>::SMEM_BYTES;
+  // the staged plain kernel: the most shared memory any launch of this tile asks for
+  const int smem = bn == 256 ? (int)GemmCfg<256, EPI_PLAIN, true>::SMEM_BYTES
+                             : (int)GemmCfg<128, EPI_PLAIN, true>::SMEM_BYTES;
   if (tile_n == 512) {
-    auto k = gemm_bf16_kernel<false, false, 256, 2, EPI_PLAIN>;
+    auto k = gemm_bf16_kernel<false, false, 256, 2, EPI_PLAIN, true>;
     B200_CHECK_CUDA(configure_smem_once((const void*)k, smem));
     *clusters = resident_clusters(k, cl, smem);
   } else if (bn == 256) {
-    auto k = gemm_bf16_kernel<false, false, 256, 1, EPI_PLAIN>;
+    auto k = gemm_bf16_kernel<false, false, 256, 1, EPI_PLAIN, true>;
     B200_CHECK_CUDA(configure_smem_once((const void*)k, smem));
     *clusters = resident_clusters(k, cl, smem);
   } else {
-    auto k = gemm_bf16_kernel<false, false, 128, 1, EPI_PLAIN>;
+    auto k = gemm_bf16_kernel<false, false, 128, 1, EPI_PLAIN, true>;
     B200_CHECK_CUDA(configure_smem_once((const void*)k, smem));
     *clusters = resident_clusters(k, cl, smem);
   }

@@ -8,7 +8,9 @@ every shape keeps its operand layouts, epilogue and LoRA second source. A decode
 step. Per frozen-base shape, in one process, alternating between the variants:
 
   ours           the shipped path, automatic tile choice
-  ours-mainloop  the same launch with the epilogue stores skipped (rlaifv_gemm_set_tuning(0, 1)): the difference to
+  ours-register  the same launch with the register epilogue (rlaifv_gemm_set_tuning(0, 2)): threads store C straight
+                 from their accumulators instead of through shared memory and TMA stores; same bits
+  ours-mainloop  the same launch with the epilogue skipped (rlaifv_gemm_set_tuning(0, 1)): the difference to
                  `ours` is the epilogue the tensor cores wait for
   cublas         torch.matmul on the same tensors and layouts (x @ W.t(), dy @ W), no fused epilogue and no second
                  source: compare it with ours-mainloop
@@ -282,11 +284,11 @@ def main(argv=None):
         f = getattr(ops, name)
         return lambda: f(*a, **kw)
 
-    def mainloop_fn(call):
+    def debug_fn(call, bits):
         g = ours_fn(call)
 
         def f():
-            L.rlaifv_gemm_set_tuning(0, 1)
+            L.rlaifv_gemm_set_tuning(0, bits)
             g()
             L.rlaifv_gemm_set_tuning(0, 0)
         return f
@@ -306,7 +308,7 @@ def main(argv=None):
     try:   # the sampler is a child process: stop it whatever happens to the timings
         for d, call, count in frozen:
             per_step = count * LAYERS              # the recorded step already holds both micro-batches
-            v = {"ours": ours_fn(call), "ours-mainloop": mainloop_fn(call)}
+            v = {"ours": ours_fn(call), "ours-register": debug_fn(call, 2), "ours-mainloop": debug_fn(call, 1)}
             if not args.no_cublas:
                 v["cublas"] = cublas_fn(call, d)
             ms = time_variants(v, args.min_seconds)
@@ -334,7 +336,8 @@ def main(argv=None):
     result["shapes"] = rows
     result["adapters"] = {"calls_per_step": ad_calls, "ms_per_step": ad_ms, "tflop_per_step": ad_fl / 1e12,
                           "tflops": ad_fl / (ad_ms * 1e-3) / 1e12 if ad_ms else None}
-    tot = {n: sum(r[n]["ms_per_step"] for r in rows if n in r) for n in ("ours", "ours-mainloop", "cublas")}
+    tot = {n: sum(r[n]["ms_per_step"] for r in rows if n in r) for n in ("ours", "ours-register", "ours-mainloop",
+                                                                            "cublas")}
     result["total_ms_per_step"] = tot
     print("frozen-base GEMMs per step: " + ", ".join("%s %.1f ms" % kv for kv in tot.items()))
     print("rank-64 adapter GEMMs per step: %d calls, %.1f ms, %.2f TFLOP" % (ad_calls, ad_ms, ad_fl / 1e12))
