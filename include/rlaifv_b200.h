@@ -7,6 +7,8 @@
  *    Nothing throws or aborts.
  *  - All pointers are raw DEVICE pointers owned by the caller (PyTorch storage in this repo);
  *    the library borrows them for the duration of the enqueued work and allocates nothing.
+ *    One exception to the first rule: rlaifv_adamw_offload_bucket also takes pinned HOST pointers (the
+ *    optimizer state the caller keeps in page-locked host memory); the caller owns those buffers too.
  *  - `stream` is a cudaStream_t (the caller's current stream); all work is enqueued asynchronously,
  *    no host synchronisation happens inside.
  *  - "bf16" = __nv_bfloat16 storage. Row-major everywhere; `ld*` = elements between rows.
@@ -271,6 +273,28 @@ int rlaifv_dpo_loss(const float* policy_win, const float* policy_rej, const floa
 int rlaifv_adamw_step(float* master, float* exp_avg, float* exp_avg_sq, const void* grad, int grad_is_f32,
                       void* param_bf16, long long n, float lr, float beta1, float beta2, float eps,
                       float weight_decay, int step, float grad_scale, void* stream);
+
+/* AdamW of one bucket whose fp32 state lives in PINNED HOST memory (the offloaded optimizer, zero2.OffloadAdamW; the
+ * DeepSpeed `offload_optimizer: {device: cpu}` of script/zero2_offload.json, with the update kept on the GPU).
+ * host_master / host_exp_avg / host_exp_avg_sq: n fp32 each, page-locked (cudaHostRegister / cudaHostAlloc) and owned
+ * by the caller; this is the one entry point that takes host pointers. grad / param_bf16: the bucket's bf16 gradient
+ * and parameters (n each, device). ring: caller-owned device staging ring of n_slots (2..8) slots, each holding
+ * master | m | v of slot_elems (% 4 == 0) floats. The state is streamed through the ring chunk by chunk: H2D on
+ * h2d_stream, the update on `stream` (same per-element arithmetic as rlaifv_adamw_step, grad_scale 1, weight decay on
+ * elements [0, decay_n)), D2H on d2h_stream, ordered by events only; with 3 slots the H2D of chunk i+1, the update of
+ * chunk i and the D2H of chunk i-1 overlap. On return, everything is enqueued: the parameters are final once `stream`
+ * reaches its current end, the host state once d2h_stream does. The caller orders h2d_stream after the previous D2H of
+ * the same host range. Pageable host or device memory where pinned host memory is expected (and host memory where
+ * device memory is expected) returns -1. The library keeps one set of events per (device, ring), created on the ring's
+ * first call; it allocates no memory. */
+int rlaifv_adamw_offload_bucket(float* host_master, float* host_exp_avg, float* host_exp_avg_sq, const void* grad,
+                                void* param_bf16, long long n, long long decay_n, float* ring, int n_slots,
+                                long long slot_elems, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                int step, void* stream, void* h2d_stream, void* d2h_stream);
+/* Destroys the events rlaifv_adamw_offload_bucket keeps for `ring` on the current device (no-op if there are none).
+ * Call it once the ring's work has completed and before the ring is freed; a later call with the same ring starts a
+ * fresh set. */
+int rlaifv_adamw_offload_release(const float* ring);
 
 #ifdef __cplusplus
 }

@@ -1,10 +1,15 @@
 // HBM-bound row kernels of the DPO step: RMSNorm / LayerNorm, RoPE, SwiGLU, CLIP patch im2col +
 // embedding assembly, image-token splice (index map + row gather/scatter), per-token log-prob
-// gather with its backward, DPO loss + gradient, fused AdamW.
+// gather with its backward, DPO loss + gradient, fused AdamW (on-device, and streamed through a
+// staging ring from pinned host memory).
 // All use 128-bit global accesses and warp-shuffle reductions; bf16 storage, fp32 math, with the
 // intermediate bf16 roundings of the HF eager path reproduced where they are observable.
 #include "common.cuh"
 #include "host_util.h"
+
+#include <map>
+#include <mutex>
+#include <utility>
 
 namespace b200 {
 
@@ -1098,6 +1103,18 @@ __global__ void dpo_loss_kernel(const float* __restrict__ pw, const float* __res
 //   g = grad*grad_scale; p *= 1-lr*wd; m = b1 m + (1-b1) g; v = b2 v + (1-b2) g^2;
 //   p -= (lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps); param_bf16 = bf16(p)
 // ------------------------------------------------------------------------------------------------
+// One element of the update. adamw_kernel and adamw_staged_kernel both call it, so the on-device and the offloaded
+// optimizer perform the same operations in the same order and their results are bit-identical.
+__device__ __forceinline__ void adamw_elem(float& p, float& m, float& v, float g, float lr, float b1, float b2,
+                                           float eps, float wd, float bc1, float bc2_sqrt, float grad_scale) {
+  const float gj = g * grad_scale;
+  p *= (1.f - lr * wd);
+  m = b1 * m + (1.f - b1) * gj;
+  v = b2 * v + (1.f - b2) * gj * gj;
+  const float denom = sqrtf(v) / bc2_sqrt + eps;
+  p -= (lr / bc1) * (m / denom);
+}
+
 template <bool GRAD_F32>
 __global__ void adamw_kernel(float* __restrict__ master, float* __restrict__ m, float* __restrict__ v,
                              const void* __restrict__ grad, bf16* __restrict__ param_out, long long n,
@@ -1121,14 +1138,39 @@ __global__ void adamw_kernel(float* __restrict__ master, float* __restrict__ m, 
     float p[4] = {p4.x, p4.y, p4.z, p4.w}, mm[4] = {m4.x, m4.y, m4.z, m4.w},
           vv[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float gj = g[j] * grad_scale;
-      p[j] *= (1.f - lr * wd);
-      mm[j] = b1 * mm[j] + (1.f - b1) * gj;
-      vv[j] = b2 * vv[j] + (1.f - b2) * gj * gj;
-      const float denom = sqrtf(vv[j]) / bc2_sqrt + eps;
-      p[j] -= (lr / bc1) * (mm[j] / denom);
-    }
+    for (int j = 0; j < 4; ++j) adamw_elem(p[j], mm[j], vv[j], g[j], lr, b1, b2, eps, wd, bc1, bc2_sqrt, grad_scale);
+    reinterpret_cast<float4*>(master)[i] = make_float4(p[0], p[1], p[2], p[3]);
+    reinterpret_cast<float4*>(m)[i] = make_float4(mm[0], mm[1], mm[2], mm[3]);
+    reinterpret_cast<float4*>(v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);
+    uint2 o;
+    o.x = pack_bf16(p[0], p[1]);
+    o.y = pack_bf16(p[2], p[3]);
+    reinterpret_cast<uint2*>(param_out)[i] = o;
+  }
+}
+
+// AdamW on one chunk of a bucket whose fp32 state was copied into a device staging slot (master | m | v, n each).
+// grad / param_out point at the chunk's first element in the bucket's bf16 gradient and parameter buffers. Elements
+// below decay_n get weight decay, the rest none, so a chunk that straddles the bucket's decay boundary is one launch
+// (a zero wd makes 1 - lr*wd exactly 1, as in the on-device path's separate no-decay launch).
+__global__ void adamw_staged_kernel(float* __restrict__ master, float* __restrict__ m, float* __restrict__ v,
+                                    const bf16* __restrict__ grad, bf16* __restrict__ param_out, long long n,
+                                    long long decay_n, float lr, float b1, float b2, float eps, float wd, float bc1,
+                                    float bc2_sqrt) {
+  const long long n4 = n >> 2;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
+       i += (long long)gridDim.x * blockDim.x) {
+    float4 p4 = reinterpret_cast<float4*>(master)[i];
+    float4 m4 = reinterpret_cast<float4*>(m)[i];
+    float4 v4 = reinterpret_cast<float4*>(v)[i];
+    uint2 u = reinterpret_cast<const uint2*>(grad)[i];
+    float2 a = unpack_bf16(u.x), b = unpack_bf16(u.y);
+    float g[4] = {a.x, a.y, b.x, b.y};
+    float p[4] = {p4.x, p4.y, p4.z, p4.w}, mm[4] = {m4.x, m4.y, m4.z, m4.w},
+          vv[4] = {v4.x, v4.y, v4.z, v4.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      adamw_elem(p[j], mm[j], vv[j], g[j], lr, b1, b2, eps, 4 * i + j < decay_n ? wd : 0.f, bc1, bc2_sqrt, 1.f);
     reinterpret_cast<float4*>(master)[i] = make_float4(p[0], p[1], p[2], p[3]);
     reinterpret_cast<float4*>(m)[i] = make_float4(mm[0], mm[1], mm[2], mm[3]);
     reinterpret_cast<float4*>(v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);
@@ -1541,6 +1583,146 @@ extern "C" int rlaifv_adamw_step(float* master, float* exp_avg, float* exp_avg_s
     adamw_kernel<false><<<grid, 256, 0, ST>>>(master, exp_avg, exp_avg_sq, grad, (bf16*)param_bf16, n, lr, beta1,
                                               beta2, eps, weight_decay, bc1, bc2_sqrt, grad_scale);
   B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- AdamW over state streamed from pinned host memory ----------------------------------------------------------------
+// Per (device, ring), one event triple per ring slot: slot s is loaded (H2D done), updated (kernel done), stored (D2H
+// done). The events outlive a call, so the first load into a slot in the next call (the next bucket) waits for the last
+// store out of it in this one, and the slot rotation carries on from call to call. They are created on a ring's first
+// call and destroyed by rlaifv_adamw_offload_release(ring), which the owner of the ring calls before freeing it.
+static constexpr int kOffloadMaxSlots = 8;
+struct OffloadEvents {
+  cudaEvent_t loaded[kOffloadMaxSlots] = {}, updated[kOffloadMaxSlots] = {}, stored[kOffloadMaxSlots] = {};
+  int next_slot = 0;
+  bool ready = false;
+};
+static std::mutex g_offload_mu;
+static std::map<std::pair<int, const float*>, OffloadEvents> g_offload_pool;
+
+static void destroy_offload_events(OffloadEvents& e) {
+  for (int s = 0; s < kOffloadMaxSlots; ++s)
+    for (cudaEvent_t* ev : {&e.loaded[s], &e.updated[s], &e.stored[s]})
+      if (*ev) {
+        cudaEventDestroy(*ev);
+        *ev = nullptr;
+      }
+  e.ready = false;
+}
+
+static int offload_events(const float* ring, OffloadEvents** out) {
+  int dev = 0;
+  B200_CHECK_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(g_offload_mu);
+  OffloadEvents& e = g_offload_pool[std::make_pair(dev, ring)];
+  if (!e.ready) {
+    cudaError_t err = cudaSuccess;
+    for (int s = 0; s < kOffloadMaxSlots && err == cudaSuccess; ++s) {
+      err = cudaEventCreateWithFlags(&e.loaded[s], cudaEventDisableTiming);
+      if (err == cudaSuccess) err = cudaEventCreateWithFlags(&e.updated[s], cudaEventDisableTiming);
+      if (err == cudaSuccess) err = cudaEventCreateWithFlags(&e.stored[s], cudaEventDisableTiming);
+    }
+    if (err != cudaSuccess) {
+      destroy_offload_events(e);
+      g_offload_pool.erase(std::make_pair(dev, ring));
+      B200_CHECK_CUDA(err);
+    }
+    e.ready = true;
+  }
+  *out = &e;
+  return 0;
+}
+
+// `what` must lie in memory of type `want` over its whole [p, p + bytes) (both ends checked).
+static int require_memory_type(const void* p, size_t bytes, cudaMemoryType want, const char* what) {
+  const char* kind = want == cudaMemoryTypeHost ? "pinned host" : "device";
+  B200_REQUIRE(p != nullptr, "adamw_offload: %s is NULL", what);
+  const void* ends[2] = {p, (const char*)p + bytes - 1};
+  for (const void* q : ends) {
+    cudaPointerAttributes a;
+    cudaError_t err = cudaPointerGetAttributes(&a, q);
+    if (err != cudaSuccess) {
+      cudaGetLastError();                 // clear it, so that the next launch's check does not report it
+      b200::set_last_error("adamw_offload: %s %p: cudaPointerGetAttributes -> %s", what, q, cudaGetErrorString(err));
+      return -1;
+    }
+    B200_REQUIRE(a.type == want, "adamw_offload: %s (%p, %zu bytes) must be %s memory (cudaMemoryType %d)", what, q,
+                 bytes, kind, (int)a.type);
+  }
+  return 0;
+}
+
+extern "C" int rlaifv_adamw_offload_bucket(float* host_master, float* host_exp_avg, float* host_exp_avg_sq,
+                                           const void* grad, void* param_bf16, long long n, long long decay_n,
+                                           float* ring, int n_slots, long long slot_elems, float lr, float beta1,
+                                           float beta2, float eps, float weight_decay, int step, void* stream,
+                                           void* h2d_stream, void* d2h_stream) {
+  B200_REQUIRE(n > 0 && n % 4 == 0 && step >= 1, "adamw_offload: n <= 0, n %% 4 != 0 or step < 1");
+  B200_REQUIRE(decay_n >= 0 && decay_n <= n, "adamw_offload: decay_n %lld outside [0, %lld]", decay_n, n);
+  B200_REQUIRE(n_slots >= 2 && n_slots <= kOffloadMaxSlots, "adamw_offload: n_slots %d outside [2, %d]", n_slots,
+               kOffloadMaxSlots);
+  B200_REQUIRE(slot_elems > 0 && slot_elems % 4 == 0, "adamw_offload: slot_elems %lld not a positive multiple of 4",
+               slot_elems);
+  B200_REQUIRE(((uintptr_t)grad & 7) == 0 && ((uintptr_t)param_bf16 & 7) == 0 && ((uintptr_t)ring & 15) == 0,
+               "adamw_offload: grad / param not 8-byte or ring not 16-byte aligned");
+  const size_t state_bytes = (size_t)n * sizeof(float);
+  int rc;
+  if ((rc = require_memory_type(host_master, state_bytes, cudaMemoryTypeHost, "host_master")) != 0) return rc;
+  if ((rc = require_memory_type(host_exp_avg, state_bytes, cudaMemoryTypeHost, "host_exp_avg")) != 0) return rc;
+  if ((rc = require_memory_type(host_exp_avg_sq, state_bytes, cudaMemoryTypeHost, "host_exp_avg_sq")) != 0) return rc;
+  if ((rc = require_memory_type(grad, (size_t)n * 2, cudaMemoryTypeDevice, "grad")) != 0) return rc;
+  if ((rc = require_memory_type(param_bf16, (size_t)n * 2, cudaMemoryTypeDevice, "param_bf16")) != 0) return rc;
+  if ((rc = require_memory_type(ring, (size_t)n_slots * 3 * slot_elems * sizeof(float), cudaMemoryTypeDevice,
+                                "ring")) != 0)
+    return rc;
+  OffloadEvents* ev = nullptr;
+  if ((rc = offload_events(ring, &ev)) != 0) return rc;
+
+  const float bc1 = 1.f - powf(beta1, (float)step);
+  const float bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
+  cudaStream_t cs = (cudaStream_t)stream, hs = (cudaStream_t)h2d_stream, ds = (cudaStream_t)d2h_stream;
+  const bf16* g = (const bf16*)grad;
+  bf16* p = (bf16*)param_bf16;
+  // chunk i: H2D on hs (after the slot's previous store), update on cs, D2H on ds. The streams run up to n_slots
+  // chunks apart, so with 3 slots the load of chunk i+1, the update of chunk i and the store of chunk i-1 overlap.
+  for (long long off = 0; off < n; off += slot_elems) {
+    const long long c = n - off < slot_elems ? n - off : slot_elems;
+    const size_t cb = (size_t)c * sizeof(float);
+    const int s = ev->next_slot % n_slots;
+    ev->next_slot = (s + 1) % n_slots;
+    float* sm = ring + (size_t)s * 3 * slot_elems;
+    float* smm = sm + slot_elems;
+    float* sv = smm + slot_elems;
+    B200_CHECK_CUDA(cudaStreamWaitEvent(hs, ev->stored[s], 0));
+    B200_CHECK_CUDA(cudaMemcpyAsync(sm, host_master + off, cb, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(smm, host_exp_avg + off, cb, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(sv, host_exp_avg_sq + off, cb, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaEventRecord(ev->loaded[s], hs));
+    B200_CHECK_CUDA(cudaStreamWaitEvent(cs, ev->loaded[s], 0));
+    long long dn = decay_n - off;
+    dn = dn < 0 ? 0 : (dn > c ? c : dn);
+    adamw_staged_kernel<<<grid_for(c / 4, 256, 16), 256, 0, cs>>>(sm, smm, sv, g + off, p + off, c, dn, lr, beta1,
+                                                                   beta2, eps, weight_decay, bc1, bc2_sqrt);
+    B200_CHECK_CUDA(cudaGetLastError());
+    B200_CHECK_CUDA(cudaEventRecord(ev->updated[s], cs));
+    B200_CHECK_CUDA(cudaStreamWaitEvent(ds, ev->updated[s], 0));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_master + off, sm, cb, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_exp_avg + off, smm, cb, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_exp_avg_sq + off, sv, cb, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaEventRecord(ev->stored[s], ds));
+  }
+  return 0;
+}
+
+extern "C" int rlaifv_adamw_offload_release(const float* ring) {
+  int dev = 0;
+  B200_CHECK_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(g_offload_mu);
+  auto it = g_offload_pool.find(std::make_pair(dev, ring));
+  if (it != g_offload_pool.end()) {
+    destroy_offload_events(it->second);
+    g_offload_pool.erase(it);
+  }
   return 0;
 }
 

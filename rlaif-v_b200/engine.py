@@ -14,7 +14,7 @@ import torch.distributed as dist
 from . import lib as _lib
 from . import ops
 from .model import LlavaDPOPolicy
-from .zero2 import Zero2AdamW, cosine_lr
+from .zero2 import OffloadAdamW, Zero2AdamW, activation_reserve_bytes, cosine_lr
 
 _F32 = torch.float32
 
@@ -27,11 +27,32 @@ class DPOStepEngine:
     def __init__(self, policy: LlavaDPOPolicy, lr=5e-7, weight_decay=0.01, betas=(0.9, 0.999), eps=1e-8,
                  total_steps=2672, warmup_ratio=0.05, dpo_use_average=False, micro_pairs=None,
                  rank=0, world=1, group=None, constant_lr=False, hf_deepspeed_input_cast=False,
-                 dpo_token_weighted=False):
+                 dpo_token_weighted=False, offload_optimizer=False, offload_budget=None, batch_pairs=None):
         self.policy = policy
         self.rank, self.world, self.group = rank, world, group
-        self.opt = Zero2AdamW(policy.trainable_buckets(), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
-                              rank=rank, world=world, group=group, gather_order=policy.param_need_order())
+        if offload_optimizer:
+            # one GPU, full fine-tuning of a model whose fp32 optimizer state does not fit next to the weights,
+            # gradients and activations: the state that does not fit is streamed from pinned host memory
+            # (zero2.OffloadAdamW; DeepSpeed offload_optimizer.device = "cpu"). offload_budget: device bytes for
+            # optimizer state. By default it is what is free after the activations of the micro-batch the step runs
+            # (micro_pairs, else the whole per-device batch `batch_pairs`) at the model's maximum sequence length
+            # (dims.max_len bounds T after the image-token splice) and the fp32 embedding-gradient buffer.
+            d = policy.dims
+            reserve = 0
+            if offload_budget is None:
+                pairs = micro_pairs or batch_pairs
+                if not pairs:
+                    raise ValueError("offload_optimizer: the device budget is sized from the micro-batch; pass "
+                                     "micro_pairs or batch_pairs (pairs per step), or an explicit offload_budget")
+                reserve = activation_reserve_bytes(d, pairs, d.max_len, getattr(policy, "stash_act", False))
+                if policy.lora is None:
+                    reserve += 4 * d.vocab_size * d.hidden_size
+            self.opt = OffloadAdamW(policy.trainable_buckets(), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
+                                    rank=rank, world=world, group=group, gather_order=policy.param_need_order(),
+                                    device_budget=offload_budget, activation_reserve=reserve)
+        else:
+            self.opt = Zero2AdamW(policy.trainable_buckets(), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
+                                  rank=rank, world=world, group=group, gather_order=policy.param_need_order())
         self.base_lr, self.total_steps, self.warmup_ratio = lr, total_steps, warmup_ratio
         self.constant_lr = constant_lr
         self.dpo_use_average = dpo_use_average

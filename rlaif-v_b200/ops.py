@@ -503,6 +503,28 @@ def adamw_step(master, exp_avg, exp_avg_sq, grad, param_bf16, lr, beta1, beta2, 
             float(eps), float(weight_decay), int(step), float(grad_scale), _l.stream_ptr())
 
 
+def adamw_offload_bucket(host_master, host_exp_avg, host_exp_avg_sq, grad, param_bf16, decay_n, ring, slot_elems, lr,
+                         beta1, beta2, eps, weight_decay, step, h2d_stream, d2h_stream):
+    """AdamW of one bucket whose fp32 state is in pinned host memory, streamed through the device staging `ring`
+    ([n_slots, 3 * slot_elems] fp32) on h2d_stream -> the current launch stream -> d2h_stream. Elements [0, decay_n)
+    get weight decay. Pinned-ness is checked by the library (a pageable tensor raises B200Error)."""
+    for t in (host_master, host_exp_avg, host_exp_avg_sq):
+        assert t.dtype == _f32 and t.device.type == "cpu" and t.is_contiguous()
+    _chk(ring, _f32), _chk(param_bf16), _chk(grad)
+    n = host_master.numel()
+    assert host_exp_avg.numel() == n and host_exp_avg_sq.numel() == n and grad.numel() == n and param_bf16.numel() == n
+    assert ring.dim() == 2 and ring.shape[1] == 3 * slot_elems
+    _l.call("rlaifv_adamw_offload_bucket", _l.ptr(host_master), _l.ptr(host_exp_avg), _l.ptr(host_exp_avg_sq),
+            _l.ptr(grad), _l.ptr(param_bf16), n, int(decay_n), _l.ptr(ring), ring.shape[0], int(slot_elems), float(lr),
+            float(beta1), float(beta2), float(eps), float(weight_decay), int(step), _l.stream_ptr(),
+            _l.c_void_p(h2d_stream.cuda_stream), _l.c_void_p(d2h_stream.cuda_stream))
+
+
+def adamw_offload_release(ring):
+    """Destroy the library's events for `ring` (call after the ring's work has completed, before freeing it)."""
+    _l.call("rlaifv_adamw_offload_release", _l.ptr(ring))
+
+
 def gemm_dual(a, b, a2, b2, out, *, k2, r, n_sub=0, b_mn=False, residual=None, accumulate=False):
     """out (+)= a @ op(b)^T + a2[:, koff:koff+k2] @ op(b2)^T (+ residual), one fp32 accumulator.
     koff = (n0 // n_sub) * r per output tile when n_sub > 0, else 0."""

@@ -8,7 +8,8 @@ Differences forced by the environment (SURVEY.md §8b "environment drift"): argu
 a small dataclass parser instead of HfArgumentParser/transformers.TrainingArguments (which refuses
 --deepspeed/--bf16 without `accelerate`), the launcher is torchrun (one process per GPU, NCCL)
 instead of `deepspeed`, and `--deepspeed <json>` is read only for its ZeRO stage (2 = what this
-engine implements natively).
+engine implements natively) and `offload_optimizer.device` ("cpu": full fine-tuning on one GPU with
+the optimizer state streamed from pinned host memory, script/zero2_offload.json).
 """
 import argparse
 import dataclasses
@@ -144,6 +145,22 @@ def zero_stage(path):
         return int(json.load(f).get("zero_optimization", {}).get("stage", 0))
 
 
+def offload_optimizer(path):
+    """DeepSpeed `zero_optimization.offload_optimizer.device` of the --deepspeed JSON: True for "cpu" (the optimizer
+    state that does not fit on the GPU lives in pinned host memory, zero2.OffloadAdamW), False when absent or "none".
+    "nvme" is not implemented."""
+    if not path:
+        return False
+    with open(path) as f:
+        block = json.load(f).get("zero_optimization", {}).get("offload_optimizer") or {}
+    device = str(block.get("device", "none")).lower()
+    if device == "nvme":
+        raise NotImplementedError("offload_optimizer.device = nvme: only \"cpu\" (pinned host memory) is implemented")
+    if device not in ("cpu", "none"):
+        raise ValueError("offload_optimizer.device = %r: expected \"cpu\" or \"none\"" % device)
+    return device == "cpu"
+
+
 def safe_save_model_for_hf_trainer(trainer, output_dir):
     """muffin/train/train_llava15.py:102-112 — full state dict to CPU, saved by the main process.
     LoRA (train_llava15_lora.py:184-197): adapter weights + `non_lora_trainables.bin` (the projector)."""
@@ -242,6 +259,7 @@ def train(attn_implementation=None, argv=None, source_rows=None):
         data_args.eval_data_source_names = data_args.eval_data_source_names.split("#")
     if zero_stage(training_args.deepspeed) not in (0, 2):
         raise NotImplementedError("only ZeRO stage 2 (script/zero2.json) is implemented natively")
+    training_args.offload_optimizer = offload_optimizer(training_args.deepspeed)
     if training_args.gradient_accumulation_steps != 1:
         # the shipped recipes use 1 (script/train/llava15_train.sh:33); inside one step the engine's own
         # --micro_pairs splits the per-device batch with gradient accumulation in the wgrad epilogues

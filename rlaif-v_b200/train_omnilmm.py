@@ -203,6 +203,7 @@ def train(argv=None, source_rows=None):
         raise NotImplementedError
     if T15.zero_stage(training_args.deepspeed) not in (0, 2, 3):
         raise NotImplementedError("unsupported ZeRO stage")
+    training_args.offload_optimizer = T15.offload_optimizer(training_args.deepspeed)
     if not omni_args.tune_clip:
         raise NotImplementedError("tune_clip=False (frozen tower): the shipped OmniLMM recipe trains the tower")
     model, data_module, tokenizer = init_model(model_args, data_args, training_args, omni_args, source_rows)

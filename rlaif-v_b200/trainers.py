@@ -26,6 +26,7 @@ import torch.distributed as dist
 
 from . import ops
 from .engine import DPOStepEngine, METRIC_NAMES
+from .zero2 import OffloadAdamW
 
 _F32 = torch.float32
 
@@ -209,6 +210,8 @@ class LLaVA15DPOTrainer:
                                     warmup_ratio=a.warmup_ratio, dpo_use_average=a.dpo_use_average,
                                     dpo_token_weighted=bool(getattr(a, "dpo_token_weighted", False)),
                                     micro_pairs=getattr(a, "micro_pairs", None), rank=self.rank, world=self.world,
+                                    offload_optimizer=bool(getattr(a, "offload_optimizer", False)),
+                                    batch_pairs=getattr(a, "per_device_train_batch_size", None),
                                     hf_deepspeed_input_cast=bool(getattr(a, "bf16", True) and getattr(a, "deepspeed", None)),
                                     constant_lr=getattr(a, "lr_scheduler_type", "cosine") == "constant")
         self.state = {"global_step": 0, "log_history": []}
@@ -414,7 +417,9 @@ class LLaVA15DPOTrainer:
             self.load_adapter(path)
         else:
             self.model.load_state_dict(torch.load(os.path.join(path, "pytorch_model.bin"), map_location="cpu"))
+        # an offloaded optimizer's state does not fit on the device: load it on the host and let it place the parts
+        offloaded = isinstance(self.engine.opt, OffloadAdamW)
         self.engine.opt.load_state_dict(torch.load(os.path.join(path, f"optimizer_rank{self.rank}.pt"),
-                                                   map_location=self.model.device))
+                                                   map_location="cpu" if offloaded else self.model.device))
         with open(os.path.join(path, "trainer_state.json")) as f:
             self.state = json.load(f)

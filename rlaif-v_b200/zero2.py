@@ -8,6 +8,8 @@ slices (12 B/param / world), gradients are reduce-scattered in place into the ow
 as a bucket's backward has finished (overlapping the rest of the backward on a side stream), the
 fused AdamW kernel updates the slice and writes bf16 straight into the parameter buffer, and an
 in-place all-gather redistributes the updated parameters.  With world == 1 the collectives vanish.
+OffloadAdamW (world == 1) keeps the state that does not fit on the device in pinned host memory and
+streams it through the GPU each step (script/zero2_offload.json).
 
 torch.distributed (NCCL) is the transport; nothing here computes on the host.
 """
@@ -69,11 +71,7 @@ class Zero2AdamW:
             self.slices.append((b, rank * n, (rank + 1) * n, total))
             total += n
         self.owned = total
-        self.master = torch.empty(total, dtype=_F32, device=dev)
-        self.exp_avg = torch.zeros(total, dtype=_F32, device=dev)
-        self.exp_avg_sq = torch.zeros(total, dtype=_F32, device=dev)
-        for b, s0, s1, o in self.slices:
-            self.master[o:o + (s1 - s0)].copy_(b.flat[s0:s1])
+        self._init_state(dev)
         self.comm_stream = torch.cuda.Stream(device=dev) if world > 1 else None
         self.opt_stream = None
         self._gathered = {}
@@ -82,6 +80,14 @@ class Zero2AdamW:
         # order in which the next forward needs the parameters (default: as given)
         self.gather_order = [self.index[n] for n in gather_order if n in self.index] if gather_order else \
             list(range(len(self.buckets)))
+
+    def _init_state(self, dev):
+        """fp32 master copy of the owned slices and zeroed moments, all on the device."""
+        self.master = torch.empty(self.owned, dtype=_F32, device=dev)
+        self.exp_avg = torch.zeros(self.owned, dtype=_F32, device=dev)
+        self.exp_avg_sq = torch.zeros(self.owned, dtype=_F32, device=dev)
+        for b, s0, s1, o in self.slices:
+            self.master[o:o + (s1 - s0)].copy_(b.flat[s0:s1])
 
     # ---- gradient reduction (called from the backward as buckets complete) ----
     def reduce_bucket(self, bucket_index):
@@ -194,3 +200,254 @@ class Zero2AdamW:
         self.master.copy_(sd["master"])
         self.exp_avg.copy_(sd["exp_avg"])
         self.exp_avg_sq.copy_(sd["exp_avg_sq"])
+
+
+# ------------------------------------------------------------------------------------------------
+# Offloaded AdamW (one GPU): the fp32 state that does not fit on the device lives in pinned host memory and is streamed
+# through a small device staging ring each step (DeepSpeed `offload_optimizer: {device: cpu}`, script/zero2_offload.json;
+# the update itself stays on the GPU). DESIGN.md §2 has the memory plan, §3 the pipeline.
+# ------------------------------------------------------------------------------------------------
+STATE_BYTES_PER_ELEM = 12            # fp32 master + exp_avg + exp_avg_sq
+DEFAULT_SLOT_ELEMS = 8 << 20         # 8 Mi elements: 96 MB per ring slot (master | m | v)
+DEFAULT_SLOTS = 3                    # load of chunk i+1 | update of chunk i | store of chunk i-1
+DEVICE_MARGIN = 2 << 30              # allocator fragmentation, CLIP tower and head buffers, library workspaces
+HOST_MARGIN = 8 << 30                # what MemAvailable must still show after the streamed state is pinned
+
+
+def offload_priority(names):
+    """Bucket names in the order they should stay on the device: the buckets whose gradients become final last first.
+    Their updates run after the whole backward and can overlap nothing; the head and the last layers finish first, so
+    their copies overlap the rest of the backward. LLaVA: embed, projector, layer0, layer1, ..., head."""
+    layers = sorted((n for n in names if n.startswith("layer") and n[5:].isdigit()), key=lambda n: int(n[5:]))
+    head = [n for n in names if n == "head"]
+    rest = [n for n in names if n not in layers and n not in head]
+    return rest + layers + head
+
+
+def offload_plan(sizes, budget_bytes, bytes_per_elem=STATE_BYTES_PER_ELEM):
+    """Resident / streamed split of the optimizer state. sizes: [(bucket name, elements)]. Buckets are taken in
+    offload_priority order while their state fits in budget_bytes; the first one that does not fit and every one after
+    it are streamed. Returns (resident names, streamed names), each in priority order."""
+    n_of = dict(sizes)
+    order = offload_priority([n for n, _ in sizes])
+    used, k = 0, 0
+    while k < len(order) and used + n_of[order[k]] * bytes_per_elem <= budget_bytes:
+        used += n_of[order[k]] * bytes_per_elem
+        k += 1
+    return order[:k], order[k:]
+
+
+def offload_chunks(n, slot_elems, decay_size):
+    """The chunks rlaifv_adamw_offload_bucket cuts a streamed bucket of n elements into: [(offset, length, elements
+    that get weight decay)]. Mirrors the loop of the C entry point (pinned by the CPU tests)."""
+    out = []
+    for off in range(0, n, slot_elems):
+        c = min(slot_elems, n - off)
+        out.append((off, c, min(c, max(0, decay_size - off))))
+    return out
+
+
+def activation_reserve_bytes(dims, pairs, seq_len, stash_act=False):
+    """Device bytes the step's activations need for `pairs` preference pairs (2 * pairs sequences) of seq_len tokens.
+    Per decoder layer and token (DESIGN.md §2): bf16 x, fused qkv, attention output, x2 and gate|up, fp32 rstd1/rstd2
+    and the attention LSE (92 KB at 7B widths), plus the SwiGLU product when it is stashed. Per token once: eight bf16
+    rows of width H for the step's working buffers."""
+    H, F, KV = dims.hidden_size, dims.intermediate_size, dims.kv_size
+    per_layer = 2 * (4 * H + 2 * KV + 2 * F) + 8 + 4 * dims.num_heads + (2 * F if stash_act else 0)
+    tokens = 2 * pairs * seq_len
+    return tokens * (per_layer * dims.num_layers + 16 * H)
+
+
+def mem_available_bytes(meminfo_text):
+    """MemAvailable of a /proc/meminfo text, in bytes (None if the line is missing)."""
+    for line in meminfo_text.splitlines():
+        if line.startswith("MemAvailable:"):
+            f = line.split()
+            return int(f[1]) * (1024 if len(f) > 2 and f[2].lower() == "kb" else 1)
+    return None
+
+
+def check_host_memory(need_bytes, meminfo_text, margin=HOST_MARGIN):
+    """Refuse (MemoryError) to pin need_bytes of optimizer state unless MemAvailable covers it plus `margin`: on a shared
+    host the kernel's OOM killer must never be the one to say no."""
+    avail = mem_available_bytes(meminfo_text)
+    if avail is None:
+        raise MemoryError("offload_optimizer: no MemAvailable line in /proc/meminfo; cannot check host memory")
+    if need_bytes + margin > avail:
+        raise MemoryError("offload_optimizer: the streamed optimizer state needs %.2f GB of pinned host memory plus a "
+                          "%.2f GB margin, but MemAvailable is %.2f GB. Give the device a larger budget, use more GPUs "
+                          "(ZeRO-2 without offload), or free host memory."
+                          % (need_bytes / 1e9, margin / 1e9, avail / 1e9))
+    return avail
+
+
+def _read_meminfo(path="/proc/meminfo"):
+    with open(path) as f:
+        return f.read()
+
+
+class OffloadAdamW(Zero2AdamW):
+    """Zero2AdamW for one GPU whose fp32 state does not all fit on the device. offload_plan keeps as many buckets'
+    state on the device as `device_budget` allows (resident buckets run the on-device path unchanged); the others'
+    state is in pinned host memory and rlaifv_adamw_offload_bucket streams it through a staging ring of n_slots x
+    slot_elems on two copy streams while the update runs on the optimizer stream. Results are bit-identical to
+    Zero2AdamW: both paths run the same per-element update (adamw_elem in rowops.cu).
+
+    device_budget: bytes of optimizer state allowed on the device. None: free device memory minus
+    `activation_reserve`, the staging ring and DEVICE_MARGIN.
+
+    Ordering: the event wait_bucket hands to the next forward is recorded after the bucket's update, not after its D2H,
+    so the copies out run under the next step's forward; a bucket's next H2D waits for its last D2H; state_dict and
+    load_state_dict wait for the copies in flight."""
+
+    def __init__(self, buckets, lr=5e-7, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, rank=0, world=1,
+                 group=None, gather_order=None, device_budget=None, activation_reserve=0,
+                 slot_elems=DEFAULT_SLOT_ELEMS, n_slots=DEFAULT_SLOTS, host_margin=HOST_MARGIN, meminfo=None):
+        if world != 1:
+            raise NotImplementedError("offload_optimizer runs on one GPU; with two or more, ZeRO-2 shards the state "
+                                      "(offloading each rank's slice is not implemented)")
+        assert slot_elems > 0 and slot_elems % 4 == 0 and 2 <= n_slots <= 8
+        self._cfg = dict(device_budget=device_budget, activation_reserve=activation_reserve, slot_elems=slot_elems,
+                         n_slots=n_slots, host_margin=host_margin, meminfo=meminfo)
+        self._host = []
+        self._stored = {}
+        self.ring = None
+        super().__init__(buckets, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, rank=rank, world=world,
+                         group=group, gather_order=gather_order)
+
+    def _init_state(self, dev):
+        cfg = self._cfg
+        largest = max(s1 - s0 for _, s0, s1, _ in self.slices)
+        self.slot_elems = min(cfg["slot_elems"], (largest + 3) // 4 * 4)
+        ring_bytes = cfg["n_slots"] * 3 * self.slot_elems * 4
+        budget = cfg["device_budget"]
+        if budget is None:
+            budget = torch.cuda.mem_get_info(dev)[0] - cfg["activation_reserve"] - ring_bytes - DEVICE_MARGIN
+        self.device_budget = budget
+        self.resident_names, self.streamed_names = offload_plan(
+            [(b.name, s1 - s0) for b, s0, s1, _ in self.slices], budget)
+        streamed = set(self.streamed_names)
+        self._global = [o for _, _, _, o in self.slices]       # offsets in the checkpoint's flat layout
+        self._is_streamed = [b.name in streamed for b, _, _, _ in self.slices]
+        local, n_dev, n_host = [], 0, 0
+        for (b, s0, s1, _), st in zip(self.slices, self._is_streamed):
+            local.append(n_host if st else n_dev)
+            if st:
+                n_host += s1 - s0
+            else:
+                n_dev += s1 - s0
+        self.resident_elems, self.streamed_elems = n_dev, n_host
+        if n_host:
+            check_host_memory(STATE_BYTES_PER_ELEM * n_host, (cfg["meminfo"] or _read_meminfo)(), cfg["host_margin"])
+        # resident buckets index the device tensors exactly as Zero2AdamW does (so _adamw_bucket is reused as is);
+        # streamed buckets index the host tensors
+        self.slices = [(b, s0, s1, lo) for (b, s0, s1, _), lo in zip(self.slices, local)]
+        self.master = torch.empty(n_dev, dtype=_F32, device=dev)
+        self.exp_avg = torch.zeros(n_dev, dtype=_F32, device=dev)
+        self.exp_avg_sq = torch.zeros(n_dev, dtype=_F32, device=dev)
+        # Plain CPU tensors of the exact size, pinned with cudaHostRegister: torch's pinned allocator rounds every block
+        # up to a power of two, which would turn ~45 GB of state into 64 GB.
+        self.host_master = torch.empty(n_host, dtype=_F32)
+        self.host_exp_avg = torch.zeros(n_host, dtype=_F32)
+        self.host_exp_avg_sq = torch.zeros(n_host, dtype=_F32)
+        for t in (self.host_master, self.host_exp_avg, self.host_exp_avg_sq):
+            if t.numel():
+                self._register(t)
+        for (b, s0, s1, o), st in zip(self.slices, self._is_streamed):
+            (self.host_master if st else self.master)[o:o + (s1 - s0)].copy_(b.flat[s0:s1])
+        if n_host:
+            self.ring = torch.empty((cfg["n_slots"], 3 * self.slot_elems), dtype=_F32, device=dev)
+            self.h2d_stream = torch.cuda.Stream(device=dev)
+            self.d2h_stream = torch.cuda.Stream(device=dev)
+        self.pinned_bytes = sum(t.numel() * 4 for t in self._host)
+
+    def _register(self, t):
+        rt = torch.cuda.cudart()
+        err = rt.cudaHostRegister(t.data_ptr(), t.numel() * t.element_size(), 0)
+        if int(err) != 0:
+            raise RuntimeError("cudaHostRegister of %.2f GB failed: %s"
+                               % (t.numel() * t.element_size() / 1e9, rt.cudaGetErrorString(err)))
+        self._host.append(t)
+
+    def close(self):
+        """Wait for the copies in flight, release the library's events for the staging ring, free the ring and unpin
+        the host state (also done when the object is collected)."""
+        if not self._host:
+            return
+        self._drain()
+        if self.ring is not None:
+            ops.adamw_offload_release(self.ring)
+            self.ring = None
+        rt = torch.cuda.cudart()
+        for t in self._host:
+            rt.cudaHostUnregister(t.data_ptr())
+        self._host = []
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _drain(self):
+        if self.ring is not None:
+            self.h2d_stream.synchronize()
+            self.d2h_stream.synchronize()
+        self._stored.clear()
+
+    def _adamw_bucket(self, bi, lr):
+        if not self._is_streamed[bi]:
+            return super()._adamw_bucket(bi, lr)
+        if not self._host:
+            raise RuntimeError("OffloadAdamW used after close()")
+        b, s0, s1, o = self.slices[bi]
+        n = s1 - s0
+        prev = self._stored.pop(bi, None)
+        if prev is not None:                 # this step's loads read what the last step's stores wrote
+            self.h2d_stream.wait_event(prev)
+        b1, b2 = self.betas
+        ops.adamw_offload_bucket(self.host_master[o:o + n], self.host_exp_avg[o:o + n], self.host_exp_avg_sq[o:o + n],
+                                 b.grad[s0:s1], b.flat[s0:s1], min(n, max(0, b.decay_size - s0)), self.ring,
+                                 self.slot_elems, lr, b1, b2, self.eps, self.wd, self.step_count, self.h2d_stream,
+                                 self.d2h_stream)
+        ev = torch.cuda.Event()
+        ev.record(self.d2h_stream)
+        self._stored[bi] = ev
+
+    def _state_parts(self):
+        return (("master", self.master, self.host_master), ("exp_avg", self.exp_avg, self.host_exp_avg),
+                ("exp_avg_sq", self.exp_avg_sq, self.host_exp_avg_sq))
+
+    def state_dict(self):
+        """The Zero2AdamW layout (full flat fp32 tensors, here on the host), so either optimizer resumes the other's
+        checkpoint. The three tensors take 12 B per parameter of host memory on top of the pinned state (81 GB at 7B):
+        MemAvailable is checked first, so a checkpoint that does not fit raises MemoryError instead of waking the
+        kernel's OOM killer."""
+        check_host_memory(STATE_BYTES_PER_ELEM * self.owned, (self._cfg["meminfo"] or _read_meminfo)(),
+                          self._cfg["host_margin"])
+        self.wait_all()
+        torch.cuda.current_stream().synchronize()
+        if self.opt_stream is not None:
+            self.opt_stream.synchronize()
+        self._drain()
+        out = {}
+        for key, dev_t, host_t in self._state_parts():
+            full = torch.empty(self.owned, dtype=_F32)
+            for (b, s0, s1, o), g, st in zip(self.slices, self._global, self._is_streamed):
+                full[g:g + (s1 - s0)].copy_((host_t if st else dev_t)[o:o + (s1 - s0)])
+            out[key] = full
+        return {"step": self.step_count, "master": out["master"], "exp_avg": out["exp_avg"],
+                "exp_avg_sq": out["exp_avg_sq"], "rank": self.rank, "world": self.world}
+
+    def load_state_dict(self, sd):
+        assert sd["world"] == self.world and sd["rank"] == self.rank
+        self.wait_all()
+        if self.opt_stream is not None:
+            self.opt_stream.synchronize()
+        self._drain()
+        self.step_count = sd["step"]
+        for key, dev_t, host_t in self._state_parts():
+            src = sd[key]
+            for (b, s0, s1, o), g, st in zip(self.slices, self._global, self._is_streamed):
+                (host_t if st else dev_t)[o:o + (s1 - s0)].copy_(src[g:g + (s1 - s0)])
+        torch.cuda.current_stream().synchronize()

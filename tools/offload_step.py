@@ -1,0 +1,332 @@
+"""Full-parameter DPO of LLaVA-1.5-7B on one GPU with the offloaded optimizer (zero2.OffloadAdamW), measured.
+
+    python tools/offload_step.py --out DIR [--skip-identity] [--skip-config-b] [--steps 5] [--warmup 3]
+
+1. Identity at real widths: LLaVA-1.5-7B dimensions at --identity-layers decoder layers (default 4). Three optimizer
+   steps with the on-device Zero2AdamW, then three from the same seed with offload and a device budget that keeps only
+   embed, projector, layer0 and layer1 resident. Reports whether the metrics, every bf16 parameter and the fp32
+   master / exp_avg / exp_avg_sq are bit-identical.
+2. Config (b): full width and depth, full fine-tuning, 8 pairs of T = 1135 (bench.py's synthetic batch), offload on,
+   with the engine's own default device budget, as the training CLI plans it with --micro_pairs --micro-pairs and
+   --model_max_length --max-len: what is free after the activations of the micro-batch at max-len and the fp32
+   embedding gradient. Step 0 (no update) is checked against ln 2, then --warmup and --steps timed steps.
+3. One JSON line (also DIR/offload_step.json): pairs/s and ms/step; resident, streamed and pinned bytes; peak device
+   memory; the optimizer's exposed time per step (end of the last backward kernel -> last update done, and -> last
+   D2H done); the H2D and D2H GB/s the streams achieved during the step; a plain cudaMemcpyAsync H2D and D2H of the
+   same pinned buffer, one direction at a time and both at the same moment on two streams; the staging ring on its
+   own (no backward beside it); the median SM clock; the GPU name and power limit.
+"""
+import argparse
+import gc
+import json
+import math
+import os
+import subprocess
+import sys
+import time
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
+
+import torch  # noqa: E402
+
+import bench  # noqa: E402  (synthetic_batch, ClockSampler, PAIRS_PER_GPU; bench.py itself is not changed)
+
+
+def parse_args(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--out", required=True)
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--micro-pairs", type=int, default=2, help="config (b)'s micro-batch (--micro_pairs of the CLI)")
+    ap.add_argument("--max-len", type=int, default=2048,
+                    help="model_max_length the engine sizes the activation reserve for (the recipe's 2048)")
+    ap.add_argument("--identity-layers", type=int, default=4)
+    ap.add_argument("--skip-identity", action="store_true")
+    ap.add_argument("--skip-config-b", action="store_true")
+    return ap.parse_args(argv)
+
+
+def gpu_name_and_power():
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30)
+        name, power = [x.strip() for x in r.stdout.strip().splitlines()[0].split(",")]
+        return name, power
+    except Exception as e:          # noqa: BLE001 — reported, not fatal
+        return "unknown (%s)" % e, None
+
+
+def make_engine(layers, micro, offload_budget=None, offload=False, seed=0):
+    from rlaifv_b200.engine import DPOStepEngine
+    from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
+    policy = LlavaDPOPolicy(LlavaDims(num_layers=layers), torch.device("cuda", 0), seed=seed)
+    eng = DPOStepEngine(policy, lr=5e-7, weight_decay=0.01, total_steps=2672, micro_pairs=micro,
+                        offload_optimizer=offload, offload_budget=offload_budget)
+    return eng
+
+
+def add_reference_logps(policy, batches, B, micro):
+    """Frozen-reference log-probs = the initial policy's (step-0 loss = ln 2), as bench.py does."""
+    for hb in batches:
+        rw, rr = [], []
+        for lo in range(0, B, micro):
+            hi = min(B, lo + micro)
+            ids = torch.cat([hb["concatenated_input_ids"][lo:hi], hb["concatenated_input_ids"][B + lo:B + hi]])
+            lab = torch.cat([hb["concatenated_labels"][lo:hi], hb["concatenated_labels"][B + lo:B + hi]])
+            out = policy.forward_logps(ids, lab, hb["images"][lo:hi], keep_stash=False)
+            rw.append(out["logp"][: hi - lo].float().cpu())
+            rr.append(out["logp"][hi - lo:].float().cpu())
+        hb["ref_win_logp"] = torch.cat(rw)
+        hb["ref_rej_logp"] = torch.cat(rr)
+
+
+def identity(layers):
+    """Three steps on the device, three offloaded from the same seed; compare everything bit for bit."""
+    from rlaifv_b200.zero2 import STATE_BYTES_PER_ELEM
+    B, micro = 4, 2
+    batches = [bench.synthetic_batch(0, s, B) for s in range(3)]
+    results = {}
+    for mode in ("device", "offload"):
+        budget = None
+        if mode == "offload":
+            budget = STATE_BYTES_PER_ELEM * sum(sizes[n] for n in ("embed", "projector", "layer0", "layer1"))
+        eng = make_engine(layers, micro, offload_budget=budget, offload=mode == "offload")
+        if mode == "device":
+            sizes = {b.name: b.size for b in eng.policy.trainable_buckets()}
+            add_reference_logps(eng.policy, batches, B, micro)
+        metrics = [eng.train_step(hb).clone() for hb in batches]
+        eng.opt.wait_all()
+        torch.cuda.synchronize()
+        sd = eng.opt.state_dict()
+        results[mode] = {"metrics": torch.stack(metrics).cpu(), "params": eng.policy.store.flat.cpu(),
+                         **{k: sd[k].cpu() for k in ("master", "exp_avg", "exp_avg_sq")}}
+        if mode == "offload":
+            split = {"resident": eng.opt.resident_names, "streamed": eng.opt.streamed_names}
+            eng.opt.close()
+        del eng, sd
+        gc.collect()                  # the policy and the engine reference each other (the backward hooks)
+        torch.cuda.empty_cache()
+    d, o = results["device"], results["offload"]
+    return {"layers": layers, "pairs": B, "micro_pairs": micro, "steps": 3, **split,
+            "metrics_identical": bool(torch.equal(d["metrics"], o["metrics"])),
+            "params_identical": bool(torch.equal(d["params"], o["params"])),
+            **{k + "_identical": bool(torch.equal(d[k], o[k])) for k in ("master", "exp_avg", "exp_avg_sq")}}
+
+
+def plain_copy_gbs(host, reps=5):
+    """cudaMemcpyAsync H2D and D2H of a pinned buffer (torch copy_ with non_blocking), CUDA-event timed."""
+    dev = torch.empty(host.numel(), dtype=host.dtype, device="cuda")
+    s = torch.cuda.Stream()
+    out = {}
+    for name, fn in (("h2d", lambda: dev.copy_(host, non_blocking=True)),
+                     ("d2h", lambda: host.copy_(dev, non_blocking=True))):
+        with torch.cuda.stream(s):
+            fn()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(s)
+            for _ in range(reps):
+                fn()
+            e1.record(s)
+        s.synchronize()
+        out[name] = reps * host.numel() * host.element_size() / (e0.elapsed_time(e1) * 1e-3) / 1e9
+    del dev
+    return out
+
+
+def concurrent_copy_gbs(host, reps=5):
+    """A plain H2D of the first half of a pinned buffer and a D2H into its second half, at the same moment on two
+    streams (the D2H writes back what the buffer held). GB/s per direction."""
+    h = host.numel() // 2
+    src, dst = host[:h], host[h:2 * h]
+    dev_in = torch.empty(h, dtype=host.dtype, device="cuda")
+    dev_out = dst.to("cuda")
+    s1, s2 = torch.cuda.Stream(), torch.cuda.Stream()
+    torch.cuda.synchronize()
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    ev[0].record(s1)
+    ev[2].record(s2)
+    with torch.cuda.stream(s1):
+        for _ in range(reps):
+            dev_in.copy_(src, non_blocking=True)
+    with torch.cuda.stream(s2):
+        for _ in range(reps):
+            dst.copy_(dev_out, non_blocking=True)
+    ev[1].record(s1)
+    ev[3].record(s2)
+    torch.cuda.synchronize()
+    b = reps * h * host.element_size()
+    out = {"h2d": b / (ev[0].elapsed_time(ev[1]) * 1e-3) / 1e9, "d2h": b / (ev[2].elapsed_time(ev[3]) * 1e-3) / 1e9}
+    del dev_in, dev_out
+    return out
+
+
+def ring_alone_gbs(opt, reps=3):
+    """rlaifv_adamw_offload_bucket on its own (no backward beside it) over a scratch range of 2^27 elements, through
+    the optimizer's staging ring: state GB/s per direction (H2D and D2H run at the same time)."""
+    from rlaifv_b200 import ops
+    n = min(1 << 27, opt.host_master.numel())
+    host = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(3)]
+    grad = torch.zeros(n, dtype=torch.bfloat16, device="cuda")
+    param = torch.zeros(n, dtype=torch.bfloat16, device="cuda")
+    s = torch.cuda.Stream()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(opt.h2d_stream)
+    from rlaifv_b200 import lib
+    with torch.cuda.stream(s), lib.use_stream(s):
+        for step in range(1, reps + 1):
+            ops.adamw_offload_bucket(*host, grad, param, n, opt.ring, opt.slot_elems, 1e-6, 0.9, 0.999, 1e-8, 0.0,
+                                     step, opt.h2d_stream, opt.d2h_stream)
+    e1.record(opt.d2h_stream)
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1)
+    del host, grad, param
+    return {"slots": opt.ring.shape[0], "slot_elems": opt.slot_elems, "elements": n, "reps": reps, "ms": ms,
+            "gbs_each_way": reps * 12 * n / (ms * 1e-3) / 1e9}
+
+
+def config_b(args):
+    """Config (b) through the engine's own default device budget, as `train_llava15.py --deepspeed
+    script/zero2_offload.json --micro_pairs M --model_max_length L` plans it."""
+    from rlaifv_b200.engine import DPOStepEngine
+    from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
+    from rlaifv_b200.zero2 import activation_reserve_bytes
+    import rlaifv_b200.zero2 as z
+    B = bench.PAIRS_PER_GPU
+    dims = LlavaDims(max_len=args.max_len)
+    T = bench.PROMPT_LEN + bench.RESP_LEN - 1 + dims.num_patches
+    micro = args.micro_pairs
+    gc.collect()
+    torch.cuda.empty_cache()
+    policy = LlavaDPOPolicy(dims, torch.device("cuda", 0), seed=0)
+    free = torch.cuda.mem_get_info()[0]
+    reserve = activation_reserve_bytes(dims, micro, dims.max_len) + 4 * dims.vocab_size * dims.hidden_size
+    t0 = time.perf_counter()
+    eng = DPOStepEngine(policy, lr=5e-7, weight_decay=0.01, total_steps=2672, micro_pairs=micro,
+                        offload_optimizer=True, batch_pairs=B)
+    setup_s = time.perf_counter() - t0
+    opt = eng.opt
+    host_batches = [bench.synthetic_batch(0, s, B) for s in range(2)]
+    add_reference_logps(policy, host_batches, B, micro)
+    batches = [{k: (v.cuda() if torch.is_tensor(v) else v) for k, v in hb.items()} for hb in host_batches]
+    while True:
+        try:
+            loss0 = float(eng.train_step(batches[0], optimizer_step=False)[0].item())
+            break
+        except torch.OutOfMemoryError:
+            policy._stash = None
+            policy._bufs.clear()
+            torch.cuda.empty_cache()
+            if micro > 1:
+                micro = max(1, micro // 2)
+                eng.micro_pairs = micro
+            else:
+                raise
+    # exposed optimizer time: the backward's last kernel is enqueued when finish_step is called
+    marks = []
+    orig_finish = opt.finish_step
+
+    def timed_finish():
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        ev[0].record(torch.cuda.current_stream())
+        orig_finish()                        # world 1: ends with the current stream waiting for every update
+        ev[1].record(torch.cuda.current_stream())
+        ev[2].record(opt.d2h_stream)
+        marks.append(ev)
+    opt.finish_step = timed_finish
+
+    def run(n):
+        for s in range(n):
+            eng.train_step(batches[s % len(batches)])
+        opt.wait_all()
+        torch.cuda.current_stream().wait_stream(opt.d2h_stream)    # the last step's stores belong to the window
+
+    run(args.warmup)
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    marks.clear()
+    sampler = bench.ClockSampler(0)
+    sampler.start()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    run(args.steps)
+    e1.record()
+    torch.cuda.synchronize()
+    clocks = sampler.stop()
+    ms = e0.elapsed_time(e1) / args.steps
+    exposed_upd = sorted(a.elapsed_time(b) for a, b, _ in marks)
+    exposed_d2h = sorted(a.elapsed_time(c) for a, _, c in marks)
+    peak_alloc, peak_reserved = torch.cuda.max_memory_allocated(), torch.cuda.max_memory_reserved()
+
+    # copy rates the streams achieved: one more step with each offloaded bucket's H2D / D2H spans event-timed
+    spans = []
+    orig_off = z.ops.adamw_offload_bucket
+
+    def timed_off(hm, *a, **kw):
+        h2d, d2h = a[-2], a[-1]
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        ev[0].record(h2d)
+        ev[2].record(d2h)
+        orig_off(hm, *a, **kw)
+        ev[1].record(h2d)
+        ev[3].record(d2h)
+        spans.append((ev, 12 * hm.numel()))
+    z.ops.adamw_offload_bucket = timed_off
+    try:
+        run(1)
+        torch.cuda.synchronize()
+    finally:
+        z.ops.adamw_offload_bucket = orig_off
+    streamed_bytes = sum(b for _, b in spans)
+    h2d_ms = sum(ev[0].elapsed_time(ev[1]) for ev, _ in spans)
+    d2h_ms = sum(ev[2].elapsed_time(ev[3]) for ev, _ in spans)
+    first_h2d, last_d2h = spans[0][0][0], spans[-1][0][3]
+    pipeline_ms = first_h2d.elapsed_time(last_d2h)
+    plain = plain_copy_gbs(opt.host_master[: min(opt.host_master.numel(), 1 << 28)])
+    plain["both_at_once"] = concurrent_copy_gbs(opt.host_master[: min(opt.host_master.numel(), 1 << 28)])
+    ring_alone = ring_alone_gbs(opt)
+    gbs = lambda b, t: b / (t * 1e-3) / 1e9 if t > 0 else None           # noqa: E731
+    med = lambda xs: xs[len(xs) // 2] if xs else None                     # noqa: E731
+    out = {
+        "pairs": B, "T": T, "micro_pairs": micro, "steps": args.steps, "warmup": args.warmup,
+        "step0_loss": loss0, "ln2": math.log(2.0), "step0_ok": abs(loss0 - math.log(2.0)) < 1e-3,
+        "ms_per_step": ms, "pairs_per_s": B / (ms * 1e-3),
+        "device_free_before_optimizer_bytes": free, "activation_reserve_bytes": reserve,
+        "device_budget_bytes": opt.device_budget, "resident_bytes": 12 * opt.resident_elems,
+        "streamed_bytes": 12 * opt.streamed_elems, "pinned_host_bytes": opt.pinned_bytes,
+        "resident_buckets": len(opt.resident_names), "streamed_buckets": len(opt.streamed_names),
+        "optimizer_setup_s": setup_s,
+        "peak_device_allocated_bytes": peak_alloc, "peak_device_reserved_bytes": peak_reserved,
+        "exposed_optimizer_ms_to_update": med(exposed_upd), "exposed_optimizer_ms_to_d2h": med(exposed_d2h),
+        "streaming": {"bytes_each_way": streamed_bytes, "h2d_busy_ms": h2d_ms, "d2h_busy_ms": d2h_ms,
+                      "h2d_gbs": gbs(streamed_bytes, h2d_ms), "d2h_gbs": gbs(streamed_bytes, d2h_ms),
+                      "first_h2d_to_last_d2h_ms": pipeline_ms},
+        "plain_copy_gbs": plain,
+        "ring_alone": ring_alone,
+        "sm_clock": clocks,
+    }
+    opt.close()
+    return out
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    os.makedirs(args.out, exist_ok=True)
+    if not torch.cuda.is_available():
+        raise SystemExit("offload_step.py measures on a GPU; no CUDA device found")
+    name, power = gpu_name_and_power()
+    line = {"gpu": name, "power_limit": power}
+    if not args.skip_identity:
+        line["identity"] = identity(args.identity_layers)
+        print(json.dumps({"identity": line["identity"]}), flush=True)
+        torch.cuda.empty_cache()
+    if not args.skip_config_b:
+        line["config_b"] = config_b(args)
+    print(json.dumps(line), flush=True)
+    with open(os.path.join(args.out, "offload_step.json"), "w") as f:
+        json.dump(line, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
