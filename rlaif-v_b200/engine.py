@@ -14,7 +14,7 @@ import torch.distributed as dist
 from . import lib as _lib
 from . import ops
 from .model import LlavaDPOPolicy
-from .zero2 import OffloadAdamW, Zero2AdamW, activation_reserve_bytes, cosine_lr
+from .zero2 import OffloadAdamW, Zero2AdamW, cosine_lr
 
 _F32 = torch.float32
 
@@ -36,7 +36,8 @@ class DPOStepEngine:
             # (zero2.OffloadAdamW; DeepSpeed offload_optimizer.device = "cpu"). offload_budget: device bytes for
             # optimizer state. By default it is what is free after the activations of the micro-batch the step runs
             # (micro_pairs, else the whole per-device batch `batch_pairs`) at the model's maximum sequence length
-            # (dims.max_len bounds T after the image-token splice) and the fp32 embedding-gradient buffer.
+            # (dims.max_len bounds T after the image-token splice) and the fp32 embedding-gradient buffer; the OmniLMM
+            # policy adds its resampler and EVA tower (policy.activation_reserve_bytes).
             d = policy.dims
             reserve = 0
             if offload_budget is None:
@@ -44,9 +45,7 @@ class DPOStepEngine:
                 if not pairs:
                     raise ValueError("offload_optimizer: the device budget is sized from the micro-batch; pass "
                                      "micro_pairs or batch_pairs (pairs per step), or an explicit offload_budget")
-                reserve = activation_reserve_bytes(d, pairs, d.max_len, getattr(policy, "stash_act", False))
-                if policy.lora is None:
-                    reserve += 4 * d.vocab_size * d.hidden_size
+                reserve = policy.activation_reserve_bytes(pairs, d.max_len)
             self.opt = OffloadAdamW(policy.trainable_buckets(), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
                                     rank=rank, world=world, group=group, gather_order=policy.param_need_order(),
                                     device_budget=offload_budget, activation_reserve=reserve)
@@ -78,6 +77,15 @@ class DPOStepEngine:
         if hasattr(policy, "on_bucket_grads_ready"):      # front-end buckets that finish inside the backward (EVA tower)
             policy.on_bucket_grads_ready = self._bucket_ready
         policy.param_ready = self.opt.wait_bucket
+
+    def load_optimizer_state(self, sd):
+        """Resume the optimizer from a state_dict of Zero2AdamW / OffloadAdamW. The policy may first refuse a checkpoint
+        written for another set of trainable parameters with a message that names the mismatch (OmniLMM: trained vs
+        frozen vision tower); the optimizer refuses any other size mismatch."""
+        check = getattr(self.policy, "check_optimizer_state", None)
+        if check is not None:
+            check(sd, self.opt.owned, self.world)
+        self.opt.load_state_dict(sd)
 
     def _layer_ready(self, layer):
         if self._last_micro:

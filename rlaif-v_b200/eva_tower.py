@@ -74,11 +74,15 @@ def pos_resample_matrix(d: EvaDims):
 
 
 class EvaTower:
-    """forward(images [B,3,S,S]) -> tokens [B, grid^2, C]; backward(d_tokens) accumulates parameter gradients."""
+    """forward(images [B,3,S,S]) -> tokens [B, grid^2, C]; backward(d_tokens) accumulates parameter gradients.
 
-    def __init__(self, dims: EvaDims, device="cuda", state=None, seed=0):
+    trainable=False (OmniLMM's `tune_clip=False`): the tower is forward-only. It has no gradient buffer and no optimizer
+    buckets, and backward() refuses."""
+
+    def __init__(self, dims: EvaDims, device="cuda", state=None, seed=0, trainable=True):
         self.dims = d = dims
         self.device = torch.device(device)
+        self.trainable = bool(trainable)
         C, Hd, HP = d.embed_dim, d.mlp_hidden, d.hp
         self.buckets = []
         off = 0
@@ -108,13 +112,14 @@ class EvaTower:
                         (f"b{i}.fc1_b", (Hd,)), (f"b{i}.fc2_b", (C,)), (f"b{i}.n2_w", (C,)), (f"b{i}.n2_b", (C,))])
         self.numel = off
         self.flat = torch.zeros(off, dtype=_BF, device=self.device)
-        self.grad = torch.zeros(off, dtype=_BF, device=self.device)
+        self.grad = torch.zeros(off, dtype=_BF, device=self.device) if self.trainable else None
         self.p, self.g = {}, {}
         for b in self.buckets:
             for s in b.segments:
                 n = math.prod(s.shape)
                 self.p[s.name] = self.flat[s.offset:s.offset + n].view(*s.shape)
-                self.g[s.name] = self.grad[s.offset:s.offset + n].view(*s.shape)
+                if self.trainable:
+                    self.g[s.name] = self.grad[s.offset:s.offset + n].view(*s.shape)
         R = pos_resample_matrix(d)                                                   # [1+N, n_pos] fp32
         Rp = torch.zeros(R.shape[0], d.n_pos_pad)
         Rp[:, : d.n_pos] = R
@@ -214,11 +219,14 @@ class EvaTower:
 
     def opt_buckets(self):
         from .zero2 import OptBucket
+        if not self.trainable:
+            return []
         return [OptBucket(b.name, self.flat[b.start:b.start + b.size], self.grad[b.start:b.start + b.size],
                           b.decay_size) for b in self.buckets]
 
     def zero_grad(self):
-        self.grad.zero_()
+        if self.trainable:
+            self.grad.zero_()
 
     def buf(self, key, shape, dtype=_BF):
         t = self._bufs.get(key)
@@ -293,6 +301,7 @@ class EvaTower:
     def backward(self, d_tokens, accumulate=False):
         """d_tokens [B, N, C] (gradient of the tower's output tokens). Parameter gradients go to `self.g`
         (overwritten unless `accumulate`)."""
+        assert self.trainable, "this tower is frozen (trainable=False): it has no backward"
         st = self._stash
         assert st is not None, "backward() needs forward(keep_stash=True)"
         d, P, G, dev = self.dims, self.p, self.g, self.device

@@ -403,6 +403,17 @@ class LlavaDPOPolicy:
             return ["projector", "embed"] + [f"layer{i}" for i in range(d.num_layers)] + ["head"]
         return ["projector"] + [f"lora{i}" for i in range(d.num_layers)]
 
+    def activation_reserve_bytes(self, pairs, seq_len):
+        """Device bytes a training micro-batch of `pairs` pairs at seq_len tokens needs next to the weights, gradients
+        and optimizer state: the decoder's activations (zero2.activation_reserve_bytes) and, in full fine-tuning, the
+        fp32 embedding-gradient buffer. The offloaded optimizer sizes its default device budget with it."""
+        from .zero2 import activation_reserve_bytes
+        d = self.dims
+        reserve = activation_reserve_bytes(d, pairs, seq_len, self.stash_act)
+        if self.lora is None:
+            reserve += 4 * d.vocab_size * d.hidden_size
+        return reserve
+
     def layer_bucket_name(self, i):
         return f"layer{i}" if self.lora is None else f"lora{i}"
 

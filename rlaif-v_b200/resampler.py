@@ -157,8 +157,10 @@ class Resampler:
     __call__ = forward
 
     # ---- backward ----
-    def backward(self, d_out):
-        """d_out [B, Q, E] -> d_x [B, N, kv_dim]; parameter gradients are ACCUMULATED into `self.g` (bf16)."""
+    def backward(self, d_out, input_grad=True):
+        """d_out [B, Q, E] -> d_x [B, N, kv_dim]; parameter gradients are ACCUMULATED into `self.g` (bf16).
+        input_grad=False (nothing upstream trains, e.g. a frozen vision tower): the backward stops at the parameters,
+        the last dgrad GEMM is skipped and None is returned."""
         st, P, G, E, Q, H = self._stash, self.p, self.g, self.embed_dim, self.num_queries, self.num_heads
         assert st is not None, "backward() needs forward(keep_stash=True)"
         B, N = st["B"], st["N"]
@@ -200,6 +202,8 @@ class Resampler:
         ops.layernorm_bwd(dxn, st["xk"], P["ln_kv.weight"], self.eps, dxk, G["ln_kv.weight"], G["ln_kv.bias"])
         # kv_proj
         ops.gemm(dxk, st["x2"], G["kv_proj.weight"], a_mn=True, b_mn=True, accumulate=True)
-        dx = ops.gemm(dxk, P["kv_proj.weight"], b_mn=True)
         self._stash = None
+        if not input_grad:
+            return None
+        dx = ops.gemm(dxk, P["kv_proj.weight"], b_mn=True)
         return dx.view(B, N, self.kv_dim)

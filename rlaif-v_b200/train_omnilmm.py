@@ -11,9 +11,19 @@ reference-log-prob dataset of the LLaVA recipe, and ZeRO (script/zero3.json for 
         --task DPO --dpo_beta 0.1 --deepspeed ./script/zero3.json --bf16 True ...
 
 Flags are those of train_llava15 (same three argument groups) plus --num_query / --image_size / --tune_clip.
-ZeRO: `--deepspeed` may name a stage-2 or stage-3 config; the engine runs its native ZeRO-2 either way: the 23 GB of
-bf16 parameters replicate on every GPU and the fp32 optimizer state is sharded (186 GB of training state in all: at
-least 4 80 GB GPUs).
+`--tune_clip False` freezes the EVA tower as the reference does (it runs forward only and is never updated; the resampler
+and the decoder train); the default `True` trains it.
+ZeRO: `--deepspeed` may name a stage-2 or stage-3 config; the engine runs its native ZeRO-2 either way: the 23.5 GB of
+bf16 parameters replicate on every GPU and the fp32 optimizer state is sharded. With the tower trained that is 11.7 B
+trainable parameters: 23.5 GB of gradients and 141 GB of fp32 state, so at N = 4 each GPU holds 23.5 + 23.5 + 35 GB
+before any activation, more than an 80 GB card; N = 8 leaves room (not measured). With `--tune_clip False` 7.3 B
+parameters train (14.7 GB of gradients, 88 GB of state).
+One GPU: `--deepspeed script/zero2_offload.json` keeps the fp32 state that does not fit in pinned host memory
+(zero2.OffloadAdamW). The device budget subtracts the activation reserve of `--micro_pairs` pairs at
+`--model_max_length` (decoder, resampler, the tower's working set and, when it trains, its stash; DESIGN.md §2). With
+`--tune_clip False --micro_pairs 2 --model_max_length 1024` on an 80 GB H100, 59 GB of state is streamed and
+MemAvailable must show 68 GB; with the tower trained (`--micro_pairs 1`) 117 GB is streamed and 126 GB is needed, which
+the optimizer refuses up front where MemAvailable is smaller.
 """
 import dataclasses
 import json
@@ -33,16 +43,17 @@ from . import train_llava15 as T15
 class OmniArguments:
     num_query: int = 64                 # omnilmm/model/omnilmm.py:46-51 (resampler queries = <im_patch> tokens per image)
     image_size: int = 448
-    tune_clip: bool = True              # the tower is trained (omnilmm.py:57-70)
+    tune_clip: bool = True              # True: the tower is trained; False: frozen, forward only (omnilmm.py:57-70)
 
 
 class OmniLMMForCausalLM:
     """Facade with the surface the trainer touches (policy, config, state_dict, train/eval)."""
 
-    def __init__(self, dims, eva_dims, device="cuda", hf_state=None, seed=0):
+    def __init__(self, dims, eva_dims, device="cuda", hf_state=None, seed=0, tune_clip=True):
         from .omnilmm_model import OmniLMMDPOPolicy
         self.dims = dims
-        self.policy = OmniLMMDPOPolicy(dims, device, hf_state=hf_state, seed=seed, eva_dims=eva_dims)
+        self.policy = OmniLMMDPOPolicy(dims, device, hf_state=hf_state, seed=seed, eva_dims=eva_dims,
+                                       tune_clip=tune_clip)
         self.device, self.dtype, self.training = self.policy.device, torch.bfloat16, True
         self.config = SimpleNamespace(hidden_size=dims.hidden_size, vocab_size=dims.vocab_size,
                                       num_hidden_layers=dims.num_layers, num_attention_heads=dims.num_heads,
@@ -178,7 +189,7 @@ def init_model(model_args, data_args, training_args, omni_args, source_rows=None
         from .omnilmm_data import DEFAULT_IMAGE_PATCH_TOKEN, DEFAULT_IM_END_TOKEN, DEFAULT_IM_START_TOKEN
         ids = tokenizer.convert_tokens_to_ids([DEFAULT_IMAGE_PATCH_TOKEN, DEFAULT_IM_START_TOKEN, DEFAULT_IM_END_TOKEN])
         dims = dataclasses.replace(dims, im_patch_token=ids[0], im_start_token=ids[1], im_end_token=ids[2])
-    model = OmniLMMForCausalLM(dims, eva, torch.device("cuda", local_rank), hf_state=state)
+    model = OmniLMMForCausalLM(dims, eva, torch.device("cuda", local_rank), hf_state=state, tune_clip=omni_args.tune_clip)
     cfg = dict(is_multimodal=True, image_token_len=dims.num_query, use_im_start_end=True,
                image_processor=SquareResizeProcessor(eva.img_size))
     train = OmniDPODataset(tokenizer, data_args.data_dir, cfg, reference_model=model, source_rows=source_rows)
@@ -204,8 +215,6 @@ def train(argv=None, source_rows=None):
     if T15.zero_stage(training_args.deepspeed) not in (0, 2, 3):
         raise NotImplementedError("unsupported ZeRO stage")
     training_args.offload_optimizer = T15.offload_optimizer(training_args.deepspeed)
-    if not omni_args.tune_clip:
-        raise NotImplementedError("tune_clip=False (frozen tower): the shipped OmniLMM recipe trains the tower")
     model, data_module, tokenizer = init_model(model_args, data_args, training_args, omni_args, source_rows)
     from .trainers import LLaVA15DPOTrainer
     training_args.model_name_or_path = model_args.model_name_or_path

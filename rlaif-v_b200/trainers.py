@@ -419,7 +419,7 @@ class LLaVA15DPOTrainer:
             self.model.load_state_dict(torch.load(os.path.join(path, "pytorch_model.bin"), map_location="cpu"))
         # an offloaded optimizer's state does not fit on the device: load it on the host and let it place the parts
         offloaded = isinstance(self.engine.opt, OffloadAdamW)
-        self.engine.opt.load_state_dict(torch.load(os.path.join(path, f"optimizer_rank{self.rank}.pt"),
-                                                   map_location="cpu" if offloaded else self.model.device))
+        self.engine.load_optimizer_state(torch.load(os.path.join(path, f"optimizer_rank{self.rank}.pt"),
+                                                    map_location="cpu" if offloaded else self.model.device))
         with open(os.path.join(path, "trainer_state.json")) as f:
             self.state = json.load(f)

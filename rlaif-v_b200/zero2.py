@@ -9,7 +9,8 @@ as a bucket's backward has finished (overlapping the rest of the backward on a s
 fused AdamW kernel updates the slice and writes bf16 straight into the parameter buffer, and an
 in-place all-gather redistributes the updated parameters.  With world == 1 the collectives vanish.
 OffloadAdamW (world == 1) keeps the state that does not fit on the device in pinned host memory and
-streams it through the GPU each step (script/zero2_offload.json).
+streams it through the GPU each step (script/zero2_offload.json); the policy's activation reserve sizes its default
+device budget (activation_reserve_bytes for the decoder, omnilmm_activation_reserve_bytes for OmniLMM).
 
 torch.distributed (NCCL) is the transport; nothing here computes on the host.
 """
@@ -194,8 +195,17 @@ class Zero2AdamW:
         return {"step": self.step_count, "master": self.master, "exp_avg": self.exp_avg,
                 "exp_avg_sq": self.exp_avg_sq, "rank": self.rank, "world": self.world}
 
+    def check_state_size(self, sd):
+        """Refuse (ValueError) a checkpoint whose flat state was written for another set of trainable buckets."""
+        n = sd["master"].numel()
+        if n != self.owned:
+            raise ValueError("optimizer checkpoint holds %d fp32 elements per state tensor, but this optimizer owns %d "
+                             "over its %d buckets (%s ...): it was written for a different set of trainable parameters"
+                             % (n, self.owned, len(self.buckets), ", ".join(b.name for b in self.buckets[:4])))
+
     def load_state_dict(self, sd):
         assert sd["world"] == self.world and sd["rank"] == self.rank
+        self.check_state_size(sd)
         self.step_count = sd["step"]
         self.master.copy_(sd["master"])
         self.exp_avg.copy_(sd["exp_avg"])
@@ -217,11 +227,20 @@ HOST_MARGIN = 8 << 30                # what MemAvailable must still show after t
 def offload_priority(names):
     """Bucket names in the order they should stay on the device: the buckets whose gradients become final last first.
     Their updates run after the whole backward and can overlap nothing; the head and the last layers finish first, so
-    their copies overlap the rest of the backward. LLaVA: embed, projector, layer0, layer1, ..., head."""
-    layers = sorted((n for n in names if n.startswith("layer") and n[5:].isdigit()), key=lambda n: int(n[5:]))
+    their copies overlap the rest of the backward. LLaVA: embed, projector, layer0, layer1, ..., head.
+    OmniLMM with a trained tower: the tail buckets embed and resampler are stepped after the whole backward; the tower's
+    backward runs after the decoder's and finishes with its embedding (eva62 first, eva_embed last), so the order is
+    embed, resampler, eva_embed, eva0, ..., eva62, layer0, ..., layer31, head. Keeping the first tower blocks resident
+    also keeps the first buckets the next forward reads off the copy streams."""
+    def numbered(prefix):
+        k = len(prefix)
+        return sorted((n for n in names if n.startswith(prefix) and n[k:].isdigit()), key=lambda n: int(n[k:]))
+    layers, eva = numbered("layer"), numbered("eva")
+    eva_embed = [n for n in names if n == "eva_embed"]
     head = [n for n in names if n == "head"]
-    rest = [n for n in names if n not in layers and n not in head]
-    return rest + layers + head
+    ordered = set(layers + eva + eva_embed + head)
+    rest = [n for n in names if n not in ordered]
+    return rest + eva_embed + eva + layers + head
 
 
 def offload_plan(sizes, budget_bytes, bytes_per_elem=STATE_BYTES_PER_ELEM):
@@ -256,6 +275,52 @@ def activation_reserve_bytes(dims, pairs, seq_len, stash_act=False):
     per_layer = 2 * (4 * H + 2 * KV + 2 * F) + 8 + 4 * dims.num_heads + (2 * F if stash_act else 0)
     tokens = 2 * pairs * seq_len
     return tokens * (per_layer * dims.num_layers + 16 * H)
+
+
+def eva_stash_bytes_per_image(e):
+    """What the trained EVA tower's forward keeps for its backward, per image (EvaTower.forward(keep_stash=True)). Per
+    live block and token (1 + grid^2 tokens): bf16 qkv (3 x padded width), attention output (padded width), the
+    attention projection, x_mid, the fc1 output, the MLP output and the block output, plus the fp32 LSE per head.
+    Once per image: the im2col columns and the embedding output (block 0's input)."""
+    S, C = e.n_tokens + 1, e.embed_dim
+    per_block = S * (2 * (4 * e.hp + 4 * C + e.mlp_hidden) + 4 * e.num_heads)
+    return e.live_blocks * per_block + e.n_tokens * 2 * e.patch_k_pad + S * 2 * C
+
+
+def eva_working_bytes_per_image(e, trained):
+    """The EVA tower's reused buffers (EvaTower._bufs, which live as long as the tower) per image, plus its output.
+    Frozen (forward without stash): qkv, attention output, attention projection, x_mid, fc1 output, MLP output, two
+    block outputs, the LayerNorm and GELU outputs and the LSE. Trained: the forward keeps only the LayerNorm and GELU
+    buffers (the rest is stash); the backward adds dy, dx (two), dm, dh, df, d(att), dqkv and the fp32 delta.
+    Both: the final LayerNorm output and the tokens without the prefix."""
+    S, C, Hd, HP = e.n_tokens + 1, e.embed_dim, e.mlp_hidden, e.hp
+    if trained:
+        elems = (C + Hd) + (5 * C + 2 * Hd + 4 * HP)
+    else:
+        elems = 4 * HP + 6 * C + 2 * Hd
+    return S * (2 * elems + 4 * e.num_heads) + S * 2 * C + e.n_tokens * 2 * C
+
+
+def resampler_bytes_per_image(dims, n_tokens):
+    """The resampler's stash and backward temporaries per image of n_tokens vision tokens (resampler.Resampler): per
+    token the bf16 input, kv_proj output, its LayerNorm, k input, k and v (stash) and dk, dv, dxn, dxk and the input
+    gradient (backward); per query row the attention output, out_proj output and ln_post output."""
+    E, W, Q = dims.hidden_size, dims.vision_width, dims.num_query
+    return n_tokens * 2 * (2 * W + 9 * E) + Q * 2 * 3 * E
+
+
+def omnilmm_activation_reserve_bytes(dims, eva, pairs, seq_len, tune_clip=True, stash_act=False):
+    """activation_reserve_bytes for the OmniLMM policy: the GQA decoder (kv_size, intermediate_size of dims) at seq_len
+    for `pairs` pairs, plus per image (one per pair) the resampler and, when the policy has its EVA tower (`eva`), the
+    tower's working set and, with tune_clip, its stash."""
+    r = activation_reserve_bytes(dims, pairs, seq_len, stash_act)
+    n_tokens = eva.n_tokens if eva is not None else 1024
+    r += pairs * resampler_bytes_per_image(dims, n_tokens)
+    if eva is not None:
+        r += pairs * eva_working_bytes_per_image(eva, tune_clip)
+        if tune_clip:
+            r += pairs * eva_stash_bytes_per_image(eva)
+    return r
 
 
 def mem_available_bytes(meminfo_text):
@@ -441,6 +506,7 @@ class OffloadAdamW(Zero2AdamW):
 
     def load_state_dict(self, sd):
         assert sd["world"] == self.world and sd["rank"] == self.rank
+        self.check_state_size(sd)
         self.wait_all()
         if self.opt_stream is not None:
             self.opt_stream.synchronize()

@@ -15,6 +15,19 @@
    D2H done); the H2D and D2H GB/s the streams achieved during the step; a plain cudaMemcpyAsync H2D and D2H of the
    same pinned buffer, one direction at a time and both at the same moment on two streams; the staging ring on its
    own (no backward beside it); the median SM clock; the GPU name and power limit.
+
+    python tools/offload_step.py --omnilmm --tune-clip {0,1} --out DIR [--max-len 1024] [--micro-pairs 2]
+
+OmniLMM-12B (config d), written to DIR/offload_step_omnilmm.json:
+1. Identity at OmniLMM widths, --identity-layers decoder layers and --identity-eva-blocks EVA blocks, in both tower
+   modes: three steps on the device, then three from the same seed offloaded with a mixed split (embed, resampler and
+   the first tower / decoder buckets resident) and with every bucket streamed. Bit identity of the metrics, the bf16
+   parameters of decoder, resampler and tower, and the fp32 master / exp_avg / exp_avg_sq; with a frozen tower, also
+   that its weights are still the initial ones.
+2. Config (d): the whole model, 8 pairs of 448 px and 512-token responses (T = 625, bench.py's OmniLMM batch), the tower
+   mode of --tune-clip, the engine's default budget for --micro-pairs at --max-len; the same report as config (b).
+3. The trained-tower recipe (--micro_pairs 1): the planner's split and the host memory it needs. It runs where
+   MemAvailable holds the streamed state; otherwise the optimizer's refusal is recorded.
 """
 import argparse
 import gc
@@ -39,12 +52,24 @@ def parse_args(argv=None):
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--micro-pairs", type=int, default=2, help="config (b)'s micro-batch (--micro_pairs of the CLI)")
-    ap.add_argument("--max-len", type=int, default=2048,
-                    help="model_max_length the engine sizes the activation reserve for (the recipe's 2048)")
+    ap.add_argument("--max-len", type=int, default=None,
+                    help="model_max_length the engine sizes the activation reserve for (default: the LLaVA recipe's "
+                         "2048; 1024 with --omnilmm)")
     ap.add_argument("--identity-layers", type=int, default=4)
     ap.add_argument("--skip-identity", action="store_true")
     ap.add_argument("--skip-config-b", action="store_true")
-    return ap.parse_args(argv)
+    ap.add_argument("--omnilmm", action="store_true",
+                    help="OmniLMM-12B (config d) instead of LLaVA-1.5-7B: identity in both tower modes, config (d) "
+                         "with the tower mode of --tune-clip, and the trained-tower plan")
+    ap.add_argument("--tune-clip", type=int, choices=(0, 1), default=0,
+                    help="with --omnilmm: 1 trains the EVA tower in the config (d) leg, 0 freezes it")
+    ap.add_argument("--identity-eva-blocks", type=int, default=4)
+    ap.add_argument("--skip-config-d", action="store_true")
+    ap.add_argument("--skip-trained-tower", action="store_true")
+    args = ap.parse_args(argv)
+    if args.max_len is None:
+        args.max_len = 1024 if args.omnilmm else 2048
+    return args
 
 
 def gpu_name_and_power():
@@ -189,25 +214,30 @@ def ring_alone_gbs(opt, reps=3):
 def config_b(args):
     """Config (b) through the engine's own default device budget, as `train_llava15.py --deepspeed
     script/zero2_offload.json --micro_pairs M --model_max_length L` plans it."""
-    from rlaifv_b200.engine import DPOStepEngine
     from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
-    from rlaifv_b200.zero2 import activation_reserve_bytes
-    import rlaifv_b200.zero2 as z
     B = bench.PAIRS_PER_GPU
     dims = LlavaDims(max_len=args.max_len)
     T = bench.PROMPT_LEN + bench.RESP_LEN - 1 + dims.num_patches
-    micro = args.micro_pairs
     gc.collect()
     torch.cuda.empty_cache()
     policy = LlavaDPOPolicy(dims, torch.device("cuda", 0), seed=0)
+    return timed_offload_run(args, policy, [bench.synthetic_batch(0, s, B) for s in range(2)], B, T)
+
+
+def timed_offload_run(args, policy, host_batches, B, T):
+    """The measured run of a full-size policy with the engine's own default device budget for --micro-pairs at
+    dims.max_len: step 0 against ln 2, --warmup and --steps timed steps, then the copy rates."""
+    from rlaifv_b200.engine import DPOStepEngine
+    import rlaifv_b200.zero2 as z
+    dims = policy.dims
+    micro = args.micro_pairs
     free = torch.cuda.mem_get_info()[0]
-    reserve = activation_reserve_bytes(dims, micro, dims.max_len) + 4 * dims.vocab_size * dims.hidden_size
+    reserve = policy.activation_reserve_bytes(micro, dims.max_len)
     t0 = time.perf_counter()
     eng = DPOStepEngine(policy, lr=5e-7, weight_decay=0.01, total_steps=2672, micro_pairs=micro,
                         offload_optimizer=True, batch_pairs=B)
     setup_s = time.perf_counter() - t0
     opt = eng.opt
-    host_batches = [bench.synthetic_batch(0, s, B) for s in range(2)]
     add_reference_logps(policy, host_batches, B, micro)
     batches = [{k: (v.cuda() if torch.is_tensor(v) else v) for k, v in hb.items()} for hb in host_batches]
     while True:
@@ -289,7 +319,7 @@ def config_b(args):
     gbs = lambda b, t: b / (t * 1e-3) / 1e9 if t > 0 else None           # noqa: E731
     med = lambda xs: xs[len(xs) // 2] if xs else None                     # noqa: E731
     out = {
-        "pairs": B, "T": T, "micro_pairs": micro, "steps": args.steps, "warmup": args.warmup,
+        "pairs": B, "T": T, "micro_pairs": micro, "max_len": dims.max_len, "steps": args.steps, "warmup": args.warmup,
         "step0_loss": loss0, "ln2": math.log(2.0), "step0_ok": abs(loss0 - math.log(2.0)) < 1e-3,
         "ms_per_step": ms, "pairs_per_s": B / (ms * 1e-3),
         "device_free_before_optimizer_bytes": free, "activation_reserve_bytes": reserve,
@@ -310,6 +340,159 @@ def config_b(args):
     return out
 
 
+# ---- OmniLMM-12B (config d) ---------------------------------------------------------------------------------------
+def omni_policy(layers, eva_blocks, tune_clip, max_len, seed=0):
+    """OmniLMM policy at real widths: `layers` decoder layers, `eva_blocks` live EVA blocks (None: all 63)."""
+    from rlaifv_b200.eva_tower import EvaDims
+    from rlaifv_b200.omnilmm_model import OmniLMMDPOPolicy, omnilmm_dims
+    dims = omnilmm_dims(num_layers=layers, max_len=max_len)
+    eva = EvaDims() if eva_blocks is None else EvaDims(depth=eva_blocks + 1)
+    return OmniLMMDPOPolicy(dims, torch.device("cuda", 0), seed=seed, eva_dims=eva, tune_clip=bool(tune_clip))
+
+
+def omni_batches(policy, B, n=2):
+    """bench.py's OmniLMM batch (T = 625) with 448 px pixels in place of the tower's tokens, as bench.py builds it."""
+    out = []
+    for s in range(n):
+        hb = bench.synthetic_omni_batch(0, s, B, policy.dims)
+        g = torch.Generator().manual_seed(4321 + s)
+        img = policy.tower.dims.img_size
+        hb["images"] = torch.randn(B, 3, img, img, generator=g).pin_memory()
+        out.append(hb)
+    return out
+
+
+def omni_snapshot(eng):
+    pol = eng.policy
+    sd = eng.opt.state_dict()
+    return {"params": torch.cat([pol.store.flat.cpu(), pol.resampler.flat.cpu(), pol.tower.flat.cpu()]),
+            **{k: sd[k].cpu() for k in ("master", "exp_avg", "exp_avg_sq")}}
+
+
+def omni_identity(layers, eva_blocks, tune_clip):
+    """OmniLMM widths at `layers` decoder layers and `eva_blocks` EVA blocks, one tower mode: three steps on the device,
+    then three offloaded from the same seed with a mixed split and with every bucket streamed."""
+    from rlaifv_b200.engine import DPOStepEngine
+    from rlaifv_b200.zero2 import STATE_BYTES_PER_ELEM
+    B, micro = 4, 2
+
+    def engine(budget):
+        pol = omni_policy(layers, eva_blocks, tune_clip, 1024)
+        return DPOStepEngine(pol, lr=5e-7, weight_decay=0.01, total_steps=2672, micro_pairs=micro,
+                             offload_optimizer=budget is not None, offload_budget=budget)
+
+    eng = engine(None)
+    sizes = {b.name: b.size for b in eng.policy.trainable_buckets()}
+    batches = omni_batches(eng.policy, B, 3)
+    add_reference_logps(eng.policy, batches, B, micro)
+    dev_metrics = torch.stack([eng.train_step(hb).clone() for hb in batches]).cpu()
+    eng.opt.wait_all()
+    torch.cuda.synchronize()
+    ref = omni_snapshot(eng)
+    tower_frozen_ok = None
+    if not tune_clip:                                    # the frozen tower's weights are the initial ones
+        tower_frozen_ok = bool(torch.equal(eng.policy.tower.flat.cpu(),
+                                           omni_policy(layers, eva_blocks, tune_clip, 1024).tower.flat.cpu()))
+    del eng
+    gc.collect()
+    torch.cuda.empty_cache()
+    first = ["embed", "resampler"] + (["eva_embed", "eva0"] if tune_clip else ["layer0"])
+    out = {"layers": layers, "eva_blocks": eva_blocks, "tune_clip": bool(tune_clip), "pairs": B, "micro_pairs": micro,
+           "steps": 3, "trainable_buckets": len(sizes), "tower_bit_unchanged": tower_frozen_ok, "splits": {}}
+    for split, budget in (("mixed", STATE_BYTES_PER_ELEM * sum(sizes[n] for n in first)), ("all_streamed", 0)):
+        eng = engine(budget)
+        metrics = torch.stack([eng.train_step(hb).clone() for hb in batches]).cpu()
+        eng.opt.wait_all()
+        torch.cuda.synchronize()
+        got = omni_snapshot(eng)
+        out["splits"][split] = {
+            "resident": eng.opt.resident_names, "streamed": len(eng.opt.streamed_names),
+            "metrics_identical": bool(torch.equal(dev_metrics, metrics)),
+            **{k + "_identical": bool(torch.equal(ref[k], got[k])) for k in ("params", "master", "exp_avg", "exp_avg_sq")}}
+        eng.opt.close()
+        del eng
+        gc.collect()
+        torch.cuda.empty_cache()
+    return out
+
+
+def mem_available():
+    from rlaifv_b200.zero2 import _read_meminfo, mem_available_bytes
+    return mem_available_bytes(_read_meminfo())
+
+
+def config_d(args, tune_clip):
+    """Config (d): the whole OmniLMM-12B (63 EVA blocks, 448 px, 32 decoder layers), 8 pairs of T = 625, through the
+    engine's own default device budget, as `train_omnilmm.py --deepspeed script/zero2_offload.json --tune_clip ...
+    --micro_pairs M --model_max_length L` plans it."""
+    gc.collect()
+    torch.cuda.empty_cache()
+    B = bench.PAIRS_PER_GPU
+    policy = omni_policy(32, None, tune_clip, args.max_len)
+    T = bench.PROMPT_LEN + bench.RESP_LEN - 1 + policy.dims.num_query + 2
+    out = timed_offload_run(args, policy, omni_batches(policy, B), B, T)
+    out["tune_clip"] = bool(tune_clip)
+    return out
+
+
+def trained_tower_plan(args):
+    """The trained-tower recipe (--micro_pairs 1): the planner's numbers, then the run itself where MemAvailable holds
+    the streamed state, otherwise the optimizer's refusal."""
+    from rlaifv_b200.engine import DPOStepEngine
+    from rlaifv_b200.zero2 import (DEFAULT_SLOT_ELEMS, DEFAULT_SLOTS, DEVICE_MARGIN, HOST_MARGIN, STATE_BYTES_PER_ELEM,
+                                   offload_plan)
+    gc.collect()
+    torch.cuda.empty_cache()
+    B, micro = bench.PAIRS_PER_GPU, 1
+    policy = omni_policy(32, None, 1, args.max_len)
+    sizes = [(b.name, b.size) for b in policy.trainable_buckets()]
+    free = torch.cuda.mem_get_info()[0]
+    reserve = policy.activation_reserve_bytes(micro, policy.dims.max_len)
+    ring = DEFAULT_SLOTS * 3 * min(DEFAULT_SLOT_ELEMS, max(n for _, n in sizes)) * 4
+    budget = free - reserve - ring - DEVICE_MARGIN
+    resident, streamed = offload_plan(sizes, budget)
+    n_of = dict(sizes)
+    streamed_bytes = STATE_BYTES_PER_ELEM * sum(n_of[n] for n in streamed)
+    plan = {"micro_pairs": micro, "max_len": policy.dims.max_len, "trainable_elems": sum(n_of.values()),
+            "device_free_before_optimizer_bytes": free, "activation_reserve_bytes": reserve,
+            "device_budget_bytes": budget, "resident_bytes": STATE_BYTES_PER_ELEM * sum(n_of[n] for n in resident),
+            "streamed_bytes": streamed_bytes, "host_needed_bytes": streamed_bytes + HOST_MARGIN,
+            "mem_available_bytes": mem_available(), "resident_buckets": len(resident), "streamed_buckets": len(streamed)}
+    try:
+        eng = DPOStepEngine(policy, offload_optimizer=True, micro_pairs=micro, batch_pairs=B)
+    except MemoryError as e:
+        plan["refused"] = str(e)
+        return plan
+    eng.opt.close()
+    del eng
+    gc.collect()
+    a = argparse.Namespace(**vars(args))
+    a.micro_pairs = micro
+    T = bench.PROMPT_LEN + bench.RESP_LEN - 1 + policy.dims.num_query + 2
+    plan["run"] = timed_offload_run(a, policy, omni_batches(policy, B), B, T)
+    return plan
+
+
+def omnilmm_main(args, line):
+    path = os.path.join(args.out, "offload_step_omnilmm.json")
+
+    def dump():
+        with open(path, "w") as f:
+            json.dump(line, f, indent=1)
+    if not args.skip_identity:
+        line["identity"] = [omni_identity(args.identity_layers, args.identity_eva_blocks, tc) for tc in (0, 1)]
+        print(json.dumps({"identity": line["identity"]}), flush=True)
+        dump()
+    if not args.skip_config_d:
+        line["config_d"] = config_d(args, args.tune_clip)
+        print(json.dumps({"config_d": line["config_d"]}), flush=True)
+        dump()
+    if not args.skip_trained_tower:
+        line["trained_tower"] = trained_tower_plan(args)
+        dump()
+    print(json.dumps(line), flush=True)
+
+
 def main(argv=None):
     args = parse_args(argv)
     os.makedirs(args.out, exist_ok=True)
@@ -317,6 +500,8 @@ def main(argv=None):
         raise SystemExit("offload_step.py measures on a GPU; no CUDA device found")
     name, power = gpu_name_and_power()
     line = {"gpu": name, "power_limit": power}
+    if args.omnilmm:
+        return omnilmm_main(args, line)
     if not args.skip_identity:
         line["identity"] = identity(args.identity_layers)
         print(json.dumps({"identity": line["identity"]}), flush=True)
