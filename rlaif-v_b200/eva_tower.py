@@ -25,17 +25,14 @@ Kernel mapping — nothing here is a new kernel family; the tower is built from 
 Parameters live in one flat bf16 buffer cut into ZeRO-2 buckets `eva_embed | eva0 .. eva62` (decay prefix = matrices,
 cls_token, pos_embed; no-decay tail = biases and LayerNorm parameters, HF Trainer's grouping).
 """
-import math
-
 import torch
 
 from . import ops
-from .model import Bucket, Segment, _round_up
+from .model import FlatStore
 
 _BF = torch.bfloat16
 _F32 = torch.float32
 PADDED_HEAD = 128
-BUCKET_PAD = 1024
 
 
 class EvaDims:
@@ -73,7 +70,7 @@ def pos_resample_matrix(d: EvaDims):
     return R
 
 
-class EvaTower:
+class EvaTower(FlatStore):
     """forward(images [B,3,S,S]) -> tokens [B, grid^2, C]; backward(d_tokens) accumulates parameter gradients.
 
     trainable=False (OmniLMM's `tune_clip=False`): the tower is forward-only. It has no gradient buffer and no optimizer
@@ -84,42 +81,15 @@ class EvaTower:
         self.device = torch.device(device)
         self.trainable = bool(trainable)
         C, Hd, HP = d.embed_dim, d.mlp_hidden, d.hp
-        self.buckets = []
-        off = 0
-
-        def add_bucket(name, decay_list, nodecay_list):
-            nonlocal off
-            b = Bucket(name=name, start=off, size=0, decay_size=0)
-            o = off
-            for nm, shape in decay_list:
-                b.segments.append(Segment(nm, shape, o, True))
-                o += math.prod(shape)
-            b.decay_size = o - off
-            for nm, shape in nodecay_list:
-                b.segments.append(Segment(nm, shape, o, False))
-                o += math.prod(shape)
-            b.size = _round_up(o - off, BUCKET_PAD)
-            off += b.size
-            self.buckets.append(b)
-
-        add_bucket("eva_embed", [("patch_w", (C, d.patch_k_pad)), ("cls", (C,)), ("pos", (d.n_pos_pad, C))],
-                   [("patch_b", (C,)), ("norm_w", (C,)), ("norm_b", (C,))])
-        for i in range(d.live_blocks):
-            add_bucket(f"eva{i}",
-                       [(f"b{i}.qkv_w", (3 * HP, C)), (f"b{i}.proj_w", (C, HP)), (f"b{i}.fc1_w", (Hd, C)),
-                        (f"b{i}.fc2_w", (C, Hd))],
-                       [(f"b{i}.qkv_b", (3 * HP,)), (f"b{i}.proj_b", (C,)), (f"b{i}.n1_w", (C,)), (f"b{i}.n1_b", (C,)),
-                        (f"b{i}.fc1_b", (Hd,)), (f"b{i}.fc2_b", (C,)), (f"b{i}.n2_w", (C,)), (f"b{i}.n2_b", (C,))])
-        self.numel = off
-        self.flat = torch.zeros(off, dtype=_BF, device=self.device)
-        self.grad = torch.zeros(off, dtype=_BF, device=self.device) if self.trainable else None
-        self.p, self.g = {}, {}
-        for b in self.buckets:
-            for s in b.segments:
-                n = math.prod(s.shape)
-                self.p[s.name] = self.flat[s.offset:s.offset + n].view(*s.shape)
-                if self.trainable:
-                    self.g[s.name] = self.grad[s.offset:s.offset + n].view(*s.shape)
+        layout = [("eva_embed", [("patch_w", (C, d.patch_k_pad)), ("cls", (C,)), ("pos", (d.n_pos_pad, C))],
+                   [("patch_b", (C,)), ("norm_w", (C,)), ("norm_b", (C,))])]
+        layout += [(f"eva{i}",
+                    [(f"b{i}.qkv_w", (3 * HP, C)), (f"b{i}.proj_w", (C, HP)), (f"b{i}.fc1_w", (Hd, C)),
+                     (f"b{i}.fc2_w", (C, Hd))],
+                    [(f"b{i}.qkv_b", (3 * HP,)), (f"b{i}.proj_b", (C,)), (f"b{i}.n1_w", (C,)), (f"b{i}.n1_b", (C,)),
+                     (f"b{i}.fc1_b", (Hd,)), (f"b{i}.fc2_b", (C,)), (f"b{i}.n2_w", (C,)), (f"b{i}.n2_b", (C,))])
+                   for i in range(d.live_blocks)]
+        super().__init__(layout, self.device, grads=self.trainable)
         R = pos_resample_matrix(d)                                                   # [1+N, n_pos] fp32
         Rp = torch.zeros(R.shape[0], d.n_pos_pad)
         Rp[:, : d.n_pos] = R
@@ -216,17 +186,6 @@ class EvaTower:
                              ("mlp.fc2.bias", "fc2_b"), ("norm2.weight", "n2_w"), ("norm2.bias", "n2_b")):
                 out[pre + src] = S[f"b{i}.{dst}"].clone()
         return out
-
-    def opt_buckets(self):
-        from .zero2 import OptBucket
-        if not self.trainable:
-            return []
-        return [OptBucket(b.name, self.flat[b.start:b.start + b.size], self.grad[b.start:b.start + b.size],
-                          b.decay_size) for b in self.buckets]
-
-    def zero_grad(self):
-        if self.trainable:
-            self.grad.zero_()
 
     def buf(self, key, shape, dtype=_BF):
         t = self._bufs.get(key)

@@ -85,10 +85,6 @@ class LlavaDims:
         return (self.patch_k + 63) // 64 * 64
 
 
-def _round_up(n, m):
-    return (n + m - 1) // m * m
-
-
 @dataclass
 class Segment:
     name: str           # storage name (fused tensors have their own names)
@@ -106,98 +102,109 @@ class Bucket:
     segments: list = field(default_factory=list)
 
 
-class ParamStore:
-    """Flat bf16 parameter / gradient storage with named views.
+class FlatStore:
+    """Flat bf16 parameter storage cut into optimizer buckets, a same-layout gradient buffer and named views of both.
+
+    layout: [(bucket name, [(segment name, shape)] with weight decay, [(segment name, shape)] without)]. A bucket is
+    its decay prefix (matrices), its no-decay tail (norms, biases), then zero padding up to a multiple of PAD.
+    `p` / `g` map segment names to views of `flat` / `grad` in segment order. grads=False (a frozen module): `grad` is
+    None, `g` is empty and there are no optimizer buckets.
+    """
+    # Zero2AdamW cuts every bucket into `world` equal slices whose length must be a multiple of 8 elements (16 B of
+    # bf16); 1024-element buckets divide that way for every power-of-two world size up to 128
+    PAD = 1024
+
+    def __init__(self, layout, device, grads=True):
+        self.buckets, off = [], 0
+        for name, decay, nodecay in layout:
+            b = Bucket(name=name, start=off, size=0, decay_size=sum(math.prod(shape) for _, shape in decay))
+            o = off
+            for segs, dec in ((decay, True), (nodecay, False)):
+                for nm, shape in segs:
+                    b.segments.append(Segment(nm, shape, o, dec))
+                    o += math.prod(shape)
+            b.size = (o - off + self.PAD - 1) // self.PAD * self.PAD
+            off += b.size
+            self.buckets.append(b)
+        self.numel = off
+        self.flat = torch.zeros(off, dtype=_BF, device=device)
+        self.grad = torch.zeros(off, dtype=_BF, device=device) if grads else None
+        self.p = self._views(self.flat)
+        self.g = self._views(self.grad) if grads else {}
+
+    def _views(self, buf):
+        return {s.name: buf[s.offset:s.offset + math.prod(s.shape)].view(s.shape)
+                for b in self.buckets for s in b.segments}
+
+    def opt_buckets(self, names=None):
+        """zero2.OptBuckets of the buckets (optionally only the named ones), in bucket order."""
+        from .zero2 import OptBucket
+        if self.grad is None:
+            return []
+        return [OptBucket(b.name, self.flat[b.start:b.start + b.size], self.grad[b.start:b.start + b.size],
+                          b.decay_size) for b in self.buckets if names is None or b.name in names]
+
+    def zero_grad(self):
+        if self.grad is not None:
+            self.grad.zero_()
+
+    def load_hf(self, state):
+        """Copy a (possibly fp32, CPU) HF-named state dict into the flat storage through the subclass's hf_views()."""
+        for k, v in self.hf_views().items():
+            v.copy_(state[k].to(device=v.device, dtype=_BF))
+
+
+class ParamStore(FlatStore):
+    """The decoder's (and LLaVA's projector's) parameters and gradients.
 
     Storage tensors: embed, per layer {qkv [3H,H], o [H,H], gu [2F,H], down [H,F], ln1 [H], ln2 [H]},
     norm [H], lm_head [V,H], projector {w0 [H,C], w2 [H,H], b0 [H], b2 [H]}.
     HF state-dict names map onto (views of) these — see hf_views().
     """
-    PAD = 1024  # bucket sizes are multiples of this (divisible by any world size <= 8 with 128-elem slices)
 
     def __init__(self, dims: LlavaDims, device):
-        self.dims = dims
-        d = dims
-        H, F, V, C = d.hidden_size, d.intermediate_size, d.vocab_size, d.clip_hidden
-        KV = d.kv_size
-        self.buckets = []
-        off = 0
-
-        def add_bucket(name, decay_list, nodecay_list):
-            nonlocal off
-            b = Bucket(name=name, start=off, size=0, decay_size=0)
-            o = off
-            for nm, shape in decay_list:
-                b.segments.append(Segment(nm, shape, o, True))
-                o += math.prod(shape)
-            b.decay_size = o - off
-            for nm, shape in nodecay_list:
-                b.segments.append(Segment(nm, shape, o, False))
-                o += math.prod(shape)
-            b.size = _round_up(o - off, self.PAD)
-            off += b.size
-            self.buckets.append(b)
-
-        add_bucket("embed", [("embed", (V, H))], [])
-        for i in range(d.num_layers):
-            add_bucket(f"layer{i}",
-                       [(f"l{i}.qkv", (H + 2 * KV, H)), (f"l{i}.o", (H, H)), (f"l{i}.gu", (2 * F, H)),
-                        (f"l{i}.down", (H, F))],
-                       [(f"l{i}.ln1", (H,)), (f"l{i}.ln2", (H,))])
-        add_bucket("head", [("lm_head", (V, H))], [("norm", (H,))])
+        self.dims = d = dims
+        H, F, V, C, KV = d.hidden_size, d.intermediate_size, d.vocab_size, d.clip_hidden, d.kv_size
+        layout = [("embed", [("embed", (V, H))], [])]
+        layout += [(f"layer{i}",
+                    [(f"l{i}.qkv", (H + 2 * KV, H)), (f"l{i}.o", (H, H)), (f"l{i}.gu", (2 * F, H)),
+                     (f"l{i}.down", (H, F))],
+                    [(f"l{i}.ln1", (H,)), (f"l{i}.ln2", (H,))]) for i in range(d.num_layers)]
+        layout.append(("head", [("lm_head", (V, H))], [("norm", (H,))]))
         if d.frontend == "clip_mlp":
-            add_bucket("projector", [("proj.w0", (H, C)), ("proj.w2", (H, H))], [("proj.b0", (H,)), ("proj.b2", (H,))])
-        self.numel = off
-        self.flat = torch.zeros(off, dtype=_BF, device=device)
-        self.grad = torch.zeros(off, dtype=_BF, device=device)
-        self.p = {}
-        self.g = {}
-        for b in self.buckets:
-            for s in b.segments:
-                n = math.prod(s.shape)
-                self.p[s.name] = self.flat[s.offset:s.offset + n].view(*s.shape)
-                self.g[s.name] = self.grad[s.offset:s.offset + n].view(*s.shape)
+            layout.append(("projector", [("proj.w0", (H, C)), ("proj.w2", (H, H))],
+                           [("proj.b0", (H,)), ("proj.b2", (H,))]))
+        super().__init__(layout, device)
 
-    def hf_views(self):
-        """HF state-dict name -> view into the fused storage (LlavaLlamaForCausalLM naming)."""
-        d = self.dims
+    def hf_views(self, grads=False):
+        """HF state-dict name -> view into the fused parameter (or, with grads, gradient) storage
+        (LlavaLlamaForCausalLM naming)."""
+        d, src = self.dims, (self.g if grads else self.p)
         H, F, KV = d.hidden_size, d.intermediate_size, d.kv_size
-        out = {"model.embed_tokens.weight": self.p["embed"], "model.norm.weight": self.p["norm"],
-               "lm_head.weight": self.p["lm_head"]}
+        out = {"model.embed_tokens.weight": src["embed"], "model.norm.weight": src["norm"],
+               "lm_head.weight": src["lm_head"]}
         if d.frontend == "clip_mlp":
-            out.update({"model.mm_projector.0.weight": self.p["proj.w0"], "model.mm_projector.0.bias": self.p["proj.b0"],
-                        "model.mm_projector.2.weight": self.p["proj.w2"], "model.mm_projector.2.bias": self.p["proj.b2"]})
+            out.update({"model.mm_projector.0.weight": src["proj.w0"], "model.mm_projector.0.bias": src["proj.b0"],
+                        "model.mm_projector.2.weight": src["proj.w2"], "model.mm_projector.2.bias": src["proj.b2"]})
         for i in range(d.num_layers):
             pre = f"model.layers.{i}."
-            qkv, gu = self.p[f"l{i}.qkv"], self.p[f"l{i}.gu"]
+            qkv, gu = src[f"l{i}.qkv"], src[f"l{i}.gu"]
             out[pre + "self_attn.q_proj.weight"] = qkv[0:H]
             out[pre + "self_attn.k_proj.weight"] = qkv[H:H + KV]
             out[pre + "self_attn.v_proj.weight"] = qkv[H + KV:H + 2 * KV]
-            out[pre + "self_attn.o_proj.weight"] = self.p[f"l{i}.o"]
+            out[pre + "self_attn.o_proj.weight"] = src[f"l{i}.o"]
             out[pre + "mlp.gate_proj.weight"] = gu[0:F]
             out[pre + "mlp.up_proj.weight"] = gu[F:2 * F]
-            out[pre + "mlp.down_proj.weight"] = self.p[f"l{i}.down"]
-            out[pre + "input_layernorm.weight"] = self.p[f"l{i}.ln1"]
-            out[pre + "post_attention_layernorm.weight"] = self.p[f"l{i}.ln2"]
+            out[pre + "mlp.down_proj.weight"] = src[f"l{i}.down"]
+            out[pre + "input_layernorm.weight"] = src[f"l{i}.ln1"]
+            out[pre + "post_attention_layernorm.weight"] = src[f"l{i}.ln2"]
         return out
 
     def hf_grad_views(self):
-        saved = self.p
-        self.p = self.g
-        try:
-            return self.hf_views()
-        finally:
-            self.p = saved
-
-    def load_hf(self, state):
-        """Copy a (possibly fp32, CPU) HF-named state dict into the flat storage."""
-        views = self.hf_views()
-        for k, v in views.items():
-            v.copy_(state[k].to(device=v.device, dtype=_BF))
+        return self.hf_views(grads=True)
 
 
-
-class LoraStore:
+class LoraStore(FlatStore):
     """Flat bf16 storage of the LoRA adapters (config e; muffin/train/train_llava15_lora.py:112-134, 304-318:
     r=64, alpha=16 on q,k,v,o,gate,up,down of every decoder layer; lm_head / projector / vision excluded).
     One bucket per layer: A_qkv [3r,H] (the three lora_A stacked — q,k,v share their input), B_q/B_k/B_v [H,r],
@@ -210,50 +217,27 @@ class LoraStore:
         self.rng_seed = 0x5EED0000 + seed
         self.step = 0                      # advanced by the engine once per optimisation step
         H, F = dims.hidden_size, dims.intermediate_size
-        self.buckets = []
-        off = 0
         shapes = [("A_qkv", (3 * r, H)), ("B_q", (H, r)), ("B_k", (H, r)), ("B_v", (H, r)), ("A_o", (r, H)),
                   ("B_o", (H, r)), ("A_gu", (2 * r, H)), ("B_g", (F, r)), ("B_u", (F, r)), ("A_d", (r, F)),
                   ("B_d", (H, r))]
-        for i in range(dims.num_layers):
-            b = Bucket(name=f"lora{i}", start=off, size=0, decay_size=0)
-            o = off
-            for nm, shape in shapes:
-                b.segments.append(Segment(f"l{i}.{nm}", shape, o, True))
-                o += math.prod(shape)
-            b.decay_size = o - off
-            b.size = _round_up(o - off, ParamStore.PAD)
-            off += b.size
-            self.buckets.append(b)
-        self.numel = off
-        self.flat = torch.zeros(off, dtype=_BF, device=device)
-        self.grad = torch.zeros(off, dtype=_BF, device=device)
-        self.p, self.g = {}, {}
-        for b in self.buckets:
-            for sg in b.segments:
-                n = math.prod(sg.shape)
-                self.p[sg.name] = self.flat[sg.offset:sg.offset + n].view(*sg.shape)
-                self.g[sg.name] = self.grad[sg.offset:sg.offset + n].view(*sg.shape)
-        for i in range(dims.num_layers):   # stacked lora_B views (adjacent segments) = second-source B operand
-            for src in (self.p, self.g):
-                q, gq = src[f"l{i}.B_q"], src[f"l{i}.B_g"]
-                base = self.flat if src is self.p else self.grad
-                oq = (q.data_ptr() - base.data_ptr()) // 2
-                og = (gq.data_ptr() - base.data_ptr()) // 2
-                src[f"l{i}.B_qkv"] = base[oq:oq + 3 * H * r].view(3 * H, r)
-                src[f"l{i}.B_gu"] = base[og:og + 2 * F * r].view(2 * F, r)
-                src[f"l{i}.B_o_cat"] = src[f"l{i}.B_o"]
-                src[f"l{i}.B_d_cat"] = src[f"l{i}.B_d"]
+        super().__init__([(f"lora{i}", [(f"l{i}.{nm}", shape) for nm, shape in shapes], [])
+                          for i in range(dims.num_layers)], device)
         # peft init: lora_A kaiming_uniform(a=sqrt(5)) = U(-1/sqrt(in), 1/sqrt(in)), lora_B = 0
         g = torch.Generator(device=device).manual_seed(seed)
-        for name, v in list(self.p.items()):
-            if name.endswith(("B_qkv", "B_gu", "B_o_cat", "B_d_cat")):
-                continue
+        for name, v in self.p.items():
             if ".A_" in name:
                 bound = 1.0 / math.sqrt(v.shape[1])
                 v.copy_((torch.rand(v.shape, generator=g, device=device) * 2 - 1) * bound)
             elif not init_b_zero:
                 v.copy_(torch.randn(v.shape, generator=g, device=device) * 0.02)
+        for i, b in enumerate(self.buckets):   # stacked lora_B views (adjacent segments) = second-source B operand
+            offset = {s.name: s.offset for s in b.segments}
+            oq, og = offset[f"l{i}.B_q"], offset[f"l{i}.B_g"]
+            for src, base in ((self.p, self.flat), (self.g, self.grad)):
+                src[f"l{i}.B_qkv"] = base[oq:oq + 3 * H * r].view(3 * H, r)
+                src[f"l{i}.B_gu"] = base[og:og + 2 * F * r].view(2 * F, r)
+                src[f"l{i}.B_o_cat"] = src[f"l{i}.B_o"]
+                src[f"l{i}.B_d_cat"] = src[f"l{i}.B_d"]
 
     _PEFT = {"q_proj": ("A_qkv", 0, "B_q"), "k_proj": ("A_qkv", 1, "B_k"), "v_proj": ("A_qkv", 2, "B_v"),
              "o_proj": ("A_o", 0, "B_o"), "gate_proj": ("A_gu", 0, "B_g"), "up_proj": ("A_gu", 1, "B_u"),
@@ -271,10 +255,6 @@ class LoraStore:
                 out[pre + "lora_A.weight"] = src[f"l{i}.{a_name}"][idx * r:(idx + 1) * r]
                 out[pre + "lora_B.weight"] = src[f"l{i}.{b_name}"]
         return out
-
-    def load_hf(self, state):
-        for k, v in self.hf_views().items():
-            v.copy_(state[k].to(device=v.device, dtype=_BF))
 
 
 class ClipWeights:
@@ -392,10 +372,9 @@ class LlavaDPOPolicy:
 
     # ---- what the optimizer trains / in which order the forward needs it ----
     def trainable_buckets(self):
-        from .zero2 import store_buckets
         if self.lora is None:
-            return store_buckets(self.store)
-        return store_buckets(self.lora) + store_buckets(self.store, names={"projector"})
+            return self.store.opt_buckets()
+        return self.lora.opt_buckets() + self.store.opt_buckets(names={"projector"})
 
     def param_need_order(self):
         d = self.dims

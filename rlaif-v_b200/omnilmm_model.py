@@ -79,9 +79,8 @@ class OmniLMMDPOPolicy(LlavaDPOPolicy):
 
     # ---- optimizer view ----
     def trainable_buckets(self):
-        from .zero2 import store_buckets
         tower = self.tower.opt_buckets() if self.tower is not None else []
-        return store_buckets(self.store) + [self.resampler.opt_bucket("resampler")] + tower
+        return self.store.opt_buckets() + self.resampler.opt_buckets() + tower
 
     def param_need_order(self):
         tower = [b.name for b in self.tower.buckets] if self.tower is not None and self.tune_clip else []

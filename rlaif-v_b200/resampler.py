@@ -12,10 +12,6 @@ The learned queries are identical for every image, so their LayerNorm, position 
 once ([Q,E] instead of [B,Q,E]); the cross-attention kernel reads that one block for every image (`q_shared`) and its
 backward's fp32 dQ reduction sums over the batch. The frozen sin-cos position table and its bicubic resize
 (`get_abs_pos`, :23-39) are constants prepared on the host at construction.
-
-Status: this is one piece of config (d). The EVA-02-E vision tower in front of it and the ZeRO-3 sharding are not
-built (DESIGN.md §6c), so the module is exercised stand-alone (tests/test_gpu_resampler.py) and is not yet wired into
-DPOStepEngine.
 """
 import math
 
@@ -23,6 +19,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .model import FlatStore
 
 _BF = torch.bfloat16
 _F32 = torch.float32
@@ -32,8 +29,6 @@ _F32 = torch.float32
 DECAY_PARAMS = ("query", "proj", "kv_proj.weight", "attn.in_proj_weight", "attn.out_proj.weight")
 NO_DECAY_PARAMS = ("attn.in_proj_bias", "attn.out_proj.bias", "ln_q.weight", "ln_q.bias", "ln_kv.weight", "ln_kv.bias",
                    "ln_post.weight", "ln_post.bias")
-PARAM_ORDER = DECAY_PARAMS + NO_DECAY_PARAMS
-BUCKET_PAD = 1024
 
 
 def _sincos_1d(dim, pos):
@@ -62,7 +57,7 @@ def resize_pos_embed(pos_embed, n_tokens):
     return t.permute(0, 2, 3, 1).flatten(0, 2)
 
 
-class Resampler:
+class Resampler(FlatStore):
     def __init__(self, grid_size, embed_dim, num_heads, kv_dim, device="cuda", state=None, seed=0, eps=1e-6):
         assert embed_dim % num_heads == 0 and embed_dim // num_heads == 128, "cross-attention kernels need head_dim 128"
         assert kv_dim % 8 == 0 and embed_dim % 8 == 0
@@ -73,17 +68,8 @@ class Resampler:
                   "attn.in_proj_bias": (3 * E,), "attn.out_proj.weight": (E, E), "attn.out_proj.bias": (E,),
                   "ln_q.weight": (E,), "ln_q.bias": (E,), "ln_kv.weight": (E,), "ln_kv.bias": (E,),
                   "ln_post.weight": (E,), "ln_post.bias": (E,)}
-        total = sum(int(np.prod(s)) for s in shapes.values())
-        self.decay_size = sum(int(np.prod(shapes[n])) for n in DECAY_PARAMS)
-        total = (total + BUCKET_PAD - 1) // BUCKET_PAD * BUCKET_PAD         # divisible by 8 * world for ZeRO-2 slices
-        self.flat = torch.zeros(total, dtype=_BF, device=self.device)      # one flat bucket (ZeRO-2 ready)
-        self.grad = torch.zeros(total, dtype=_BF, device=self.device)
-        self.p, self.g, off = {}, {}, 0
-        for name in PARAM_ORDER:
-            n = int(np.prod(shapes[name]))
-            self.p[name] = self.flat[off:off + n].view(shapes[name])
-            self.g[name] = self.grad[off:off + n].view(shapes[name])
-            off += n
+        super().__init__([("resampler", [(n, shapes[n]) for n in DECAY_PARAMS],
+                           [(n, shapes[n]) for n in NO_DECAY_PARAMS])], self.device)
         pos = sincos_pos_embed(E, grid_size)
         if state is not None:
             self.load_state_dict(state)
@@ -114,14 +100,6 @@ class Resampler:
     def load_state_dict(self, state):
         for k, v in self.p.items():
             v.copy_(state[k].to(device=self.device, dtype=_BF))
-
-    def zero_grad(self):
-        self.grad.zero_()
-
-    def opt_bucket(self, name="resampler"):
-        """The whole module as one ZeRO-2 / AdamW bucket (zero2.OptBucket)."""
-        from .zero2 import OptBucket
-        return OptBucket(name, self.flat, self.grad, self.decay_size)
 
     def _pos_for(self, n_tokens):
         if n_tokens not in self._pos_kv:

@@ -43,21 +43,9 @@ class OptBucket:
         self.size = flat.numel()
 
 
-def store_buckets(store, names=None):
-    """OptBuckets of a ParamStore / LoraStore (optionally only the named ones)."""
-    out = []
-    for b in store.buckets:
-        if names is None or b.name in names:
-            out.append(OptBucket(b.name, store.flat[b.start:b.start + b.size], store.grad[b.start:b.start + b.size],
-                                 b.decay_size))
-    return out
-
-
 class Zero2AdamW:
     def __init__(self, buckets, lr=5e-7, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, rank=0, world=1,
                  group=None, gather_order=None):
-        if not isinstance(buckets, (list, tuple)):         # a ParamStore: every bucket is trainable
-            buckets = store_buckets(buckets)
         self.buckets = list(buckets)
         self.index = {b.name: i for i, b in enumerate(self.buckets)}
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay

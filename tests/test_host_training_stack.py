@@ -147,7 +147,7 @@ GLOO_WORKER = textwrap.dedent('''
     x0 = xflat.clone().float()
     torch.manual_seed(200 + rank); xgrad.copy_((torch.randn(2048) * 0.5).bfloat16())
     xsum = xgrad.float().clone(); dist.all_reduce(xsum)
-    buckets = zero2.store_buckets(st) + [zero2.OptBucket("resampler", xflat, xgrad, 1024)]
+    buckets = st.opt_buckets() + [zero2.OptBucket("resampler", xflat, xgrad, 1024)]
     opt = zero2.Zero2AdamW(buckets, lr=0.1, weight_decay=0.0, rank=rank, world=world,
                            gather_order=["resampler", "embed", "layer0", "layer1", "head", "projector"])
     assert opt.owned * world == st.numel + 2048 and opt.index["resampler"] == len(buckets) - 1
