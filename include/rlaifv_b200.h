@@ -224,8 +224,7 @@ int rlaifv_f32_to_bf16_2d(const float* in, long long ld_in, void* out, long long
  * the log-softmax only need those rows (512 of 1135 per config-(b) sequence). row_pos int32 [nseq*cap]:
  * row_pos[s*cap + j] = s*T + t of sequence s's j-th supervised position, -1 in unused slots (cap >= labels per row).
  * rows_gather: out[r] = x[row_pos[r]] (zeros for -1); rows_scatter: dx[row_pos[r]] = dy[r] (dx pre-zeroed).
- * logp_fwd_rows / logp_bwd_rows: the log-prob gather and its in-place backward on logits [n_rows][ld] of the gathered
- * rows; per_tok [nseq][T-1] pre-zeroed, lse [n_rows]; token_weight / norm nullable (token-weighted and average modes). */
+ * rlaifv_logp_fwd / rlaifv_logp_bwd take this row_pos to run the log-prob head on the gathered rows. */
 /* Token weights [nseq][Lw] in TEXT positions (collator: weight i belongs to token i+1) -> [nseq][T-1] in SPLICED
  * positions via the splice map src [nseq][T] (image rows / padding -> 1). Extension beyond the reference, which refuses
  * --dpo_token_weighted for LLaVA-1.5 (muffin/train/trainers.py:246-248). */
@@ -233,32 +232,29 @@ int rlaifv_splice_token_weight(const int* src, const float* token_weight, float*
 int rlaifv_supervised_rows(const long long* labels, int nseq, int T, int cap, int* row_pos, void* stream);
 int rlaifv_rows_gather(const int* row_pos, const void* x, void* out, long long n_rows, int H, void* stream);
 int rlaifv_rows_scatter(const int* row_pos, const void* dy, void* dx, long long n_rows, int H, void* stream);
-int rlaifv_logp_fwd_rows(const void* logits, long long ld, const long long* labels, const int* row_pos, long long n_rows,
-                         int nseq, int T, int V, float* per_tok, float* lse, float* logp_sum, float* logp_avg,
-                         float* count, void* stream);
-int rlaifv_logp_bwd_rows(void* logits, long long ld, const long long* labels, const int* row_pos, long long n_rows,
-                         const float* lse, const float* d_logp, const float* token_weight, const float* norm, int nseq,
-                         int T, int V, void* stream);
 
 /* ---- per-token log-prob gather (muffin/eval/muffin_inference_logp.py:82-115) ---------------------
- * logits bf16 [nseq*T][ld] (upcast to fp32 inside, as pinned transformers 4.35 does), labels = spliced
- * labels [nseq][T]. per_tok [nseq][T-1], lse [nseq][T], logp_sum/logp_avg/count [nseq].
- * logp_bwd overwrites logits with d loss / d logits given d loss / d logp_sum (count != NULL:
- * average mode). */
-int rlaifv_logp_fwd(const void* logits, long long ld, const long long* labels, int nseq, int T, int V,
-                    float* per_tok, float* lse, float* logp_sum, float* logp_avg, float* count, void* stream);
-int rlaifv_logp_bwd(void* logits, long long ld, const long long* labels, const float* lse, const float* d_logp,
-                    const float* count_or_null, int nseq, int T, int V, void* stream);
+ * logits bf16, upcast to fp32 inside as pinned transformers 4.35 does; labels = spliced labels [nseq][T].
+ * row_pos NULL: the full head, logits [nseq*T][ld], lse [nseq][T]. row_pos given: the compact head above, logits
+ * [n_rows][ld] of the gathered rows, lse [n_rows], per_tok pre-zeroed by the caller. per_tok [nseq][T-1],
+ * logp_sum/logp_avg/count [nseq].
+ * logp_bwd overwrites logits with d loss / d logits given d loss / d logp_sum, in the same layout. token_weight
+ * (nullable) scales each row by its weight (the token-weighted loss below); norm != NULL is average mode: the label
+ * count, or the weight sum when weighted. */
+int rlaifv_logp_fwd(const void* logits, long long ld, const long long* labels, const int* row_pos, long long n_rows,
+                    int nseq, int T, int V, float* per_tok, float* lse, float* logp_sum, float* logp_avg, float* count,
+                    void* stream);
+int rlaifv_logp_bwd(void* logits, long long ld, const long long* labels, const int* row_pos, long long n_rows,
+                    const float* lse, const float* d_logp, const float* token_weight, const float* norm, int nseq,
+                    int T, int V, void* stream);
 
-/* Token-weighted log-prob reduction and its backward: compute_weighted_logp (muffin/train/trainers.py:128-137), used by
- * the `dpo_token_weighted` branch of get_beta_and_logps (:246-261; the reference raises NotImplementedError for
- * LLaVA-1.5 there, so this serves the OmniLMM path). token_weight fp32 [nseq][T-1]; weighted_mask = weight * (label !=
- * -100); logp_w = sum per_tok * weighted_mask, avg_w = logp_w / sum weighted_mask (wsum). Backward in place on the logits
- * like rlaifv_logp_bwd, each row scaled by its token weight (and 1/wsum in average mode). */
+/* Token-weighted log-prob reduction: compute_weighted_logp (muffin/train/trainers.py:128-137), used by the
+ * `dpo_token_weighted` branch of get_beta_and_logps (:246-261; the reference raises NotImplementedError for LLaVA-1.5
+ * there, so this serves the OmniLMM path). token_weight fp32 [nseq][T-1]; weighted_mask = weight * (label != -100);
+ * logp_w = sum per_tok * weighted_mask, avg_w = logp_w / sum weighted_mask (wsum). Its backward is rlaifv_logp_bwd
+ * with token_weight (and norm = wsum in average mode). */
 int rlaifv_logp_weighted_reduce(const float* per_tok, const long long* labels, const float* token_weight, int nseq,
                                 int T, float* logp_w, float* avg_w, float* wsum_or_null, void* stream);
-int rlaifv_logp_bwd_weighted(void* logits, long long ld, const long long* labels, const float* lse, const float* d_logp,
-                             const float* token_weight, const float* wsum_or_null, int nseq, int T, int V, void* stream);
 
 /* ---- DPO loss + gradient (muffin/train/trainers.py:91-126, :279-311) ---------------------------
  * out9: [0] loss = DPO_w*mean(losses) - SFT_w*mean(pw); [1..8] local means of chosen_reward,

@@ -873,16 +873,23 @@ logp_fwd_kernel(const bf16* __restrict__ logits, long long ld, const long long* 
     }
   }
 }
-// per-sequence reductions: logp_sum[b] = sum_t per_tok*mask ; avg = sum / count
-__global__ void logp_reduce_kernel(const float* __restrict__ per_tok,
-                                   const long long* __restrict__ labels, int nseq, int T,
+// Per-sequence reductions. Token-weighted when token_weight [nseq][T-1] is given (compute_weighted_logp,
+// muffin/train/trainers.py:128-137 — the `dpo_token_weighted` branch of get_beta_and_logps, :246-261), weight 1 when
+// it is nullptr: mask = weight * (label != -100); logp_sum[b] = sum_t per_tok * mask; count[b] = sum_t mask;
+// avg = logp_sum / count. A weight of exactly 1 rounds like the plain sum (fma(p, 1, s) == p + s).
+__global__ void logp_reduce_kernel(const float* __restrict__ per_tok, const long long* __restrict__ labels,
+                                   const float* __restrict__ token_weight, int nseq, int T,
                                    float* __restrict__ logp_sum, float* __restrict__ logp_avg,
                                    float* __restrict__ count_out) {
   const int b = blockIdx.x;
   float s = 0.f, c = 0.f;
   for (int t = threadIdx.x; t < T - 1; t += blockDim.x) {
     const bool mk = labels[(long long)b * T + t + 1] != IGNORE_INDEX;
-    if (mk) { s += per_tok[(long long)b * (T - 1) + t]; c += 1.f; }
+    if (mk) {
+      const float w = token_weight ? token_weight[(long long)b * (T - 1) + t] : 1.f;
+      s += per_tok[(long long)b * (T - 1) + t] * w;
+      c += w;
+    }
   }
   const float2 tot = block_sum2(s, c);
   if (threadIdx.x == 0) {
@@ -891,73 +898,16 @@ __global__ void logp_reduce_kernel(const float* __restrict__ per_tok,
     if (count_out) count_out[b] = tot.y;
   }
 }
-// backward, in place: logits[b][t][v] <- g_b * mask * (onehot(v==label) - softmax_v), row T-1 <- 0.
-// g_b = d_logp[b] (sum mode) or d_logp[b]/count[b] (average mode, count passed non-null).
+// backward, in place: logits[b][t][v] <- g_b * w[b][t] * mask * (onehot(v==label) - softmax_v), row T-1 <- 0;
+// w = token_weight (1 when nullptr); g_b = d_logp[b] (sum mode) or d_logp[b] / norm[b] (average mode, norm passed
+// non-null: the label count, or the weight sum when weighted).
 __global__ void __launch_bounds__(LOGP_THREADS)
 logp_bwd_kernel(bf16* __restrict__ logits, long long ld, const long long* __restrict__ labels,
                 const float* __restrict__ lse, const float* __restrict__ d_logp,
-                const float* __restrict__ count, int nseq, int T, int V) {
-  const long long rows = (long long)nseq * T;
-  const int nch = V >> 3;
-  for (long long r = blockIdx.x; r < rows; r += gridDim.x) {
-    const int b = (int)(r / T);
-    const int t = (int)(r % T);
-    bf16* lr = logits + r * ld;
-    long long lab = (t < T - 1) ? labels[(long long)b * T + t + 1] : IGNORE_INDEX;
-    if (lab == IGNORE_INDEX) {
-      for (int c = threadIdx.x; c < nch; c += LOGP_THREADS)
-        *reinterpret_cast<uint4*>(lr + c * 8) = make_uint4(0, 0, 0, 0);
-      continue;
-    }
-    float g = d_logp[b];
-    if (count) g /= count[b];
-    const float l = lse[r];
-    for (int c = threadIdx.x; c < nch; c += LOGP_THREADS) {
-      float v[8];
-      load8(lr + c * 8, v);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float p = __expf(v[j] - l);
-        v[j] = g * (((long long)(c * 8 + j) == lab ? 1.f : 0.f) - p);
-      }
-      store8(lr + c * 8, v);
-    }
-  }
-}
-
-// Token-weighted variant (compute_weighted_logp, muffin/train/trainers.py:128-137 — the `dpo_token_weighted` branch of
-// get_beta_and_logps, :246-261, available to the non-LLaVA models): weighted_mask = token_weight * (label != -100);
-// logp_w[b] = sum_t per_tok * weighted_mask; avg_w = logp_w / sum_t weighted_mask. token_weight is [nseq][T-1].
-__global__ void logp_weighted_reduce_kernel(const float* __restrict__ per_tok, const long long* __restrict__ labels,
-                                            const float* __restrict__ token_weight, int nseq, int T,
-                                            float* __restrict__ logp_w, float* __restrict__ avg_w,
-                                            float* __restrict__ wsum_out) {
-  const int b = blockIdx.x;
-  float s = 0.f, c = 0.f;
-  for (int t = threadIdx.x; t < T - 1; t += blockDim.x) {
-    const bool mk = labels[(long long)b * T + t + 1] != IGNORE_INDEX;
-    if (mk) {
-      const float w = token_weight[(long long)b * (T - 1) + t];
-      s += per_tok[(long long)b * (T - 1) + t] * w;
-      c += w;
-    }
-  }
-  const float2 tot = block_sum2(s, c);
-  if (threadIdx.x == 0) {
-    logp_w[b] = tot.x;
-    avg_w[b] = tot.x / tot.y;
-    if (wsum_out) wsum_out[b] = tot.y;
-  }
-}
-// backward of the weighted sum, in place: logits[b][t][v] <- g_b * w[b][t] * mask * (onehot - softmax), row T-1 <- 0;
-// g_b = d_logp[b] (sum mode) or d_logp[b] / wsum[b] (average mode, wsum passed non-null).
-__global__ void __launch_bounds__(LOGP_THREADS)
-logp_bwd_weighted_kernel(bf16* __restrict__ logits, long long ld, const long long* __restrict__ labels,
-                         const float* __restrict__ lse, const float* __restrict__ d_logp,
-                         const float* __restrict__ token_weight, const float* __restrict__ wsum, int nseq, int T,
-                         int V, const int* __restrict__ row_pos, long long n_compact) {
-  // token_weight may be nullptr (plain sum / average: wsum is then the label count); row_pos: compact head (see
-  // logp_fwd_kernel) — logits row r is position row_pos[r], padding slots and unsupervised rows are zeroed.
+                const float* __restrict__ token_weight, const float* __restrict__ norm, int nseq, int T,
+                int V, const int* __restrict__ row_pos, long long n_compact) {
+  // row_pos: compact head (see logp_fwd_kernel) — logits row r is position row_pos[r], padding slots and unsupervised
+  // rows are zeroed.
   const long long rows = row_pos ? n_compact : (long long)nseq * T;
   const int nch = V >> 3;
   for (long long r = blockIdx.x; r < rows; r += gridDim.x) {
@@ -978,7 +928,7 @@ logp_bwd_weighted_kernel(bf16* __restrict__ logits, long long ld, const long lon
       continue;
     }
     float g = d_logp[b] * (token_weight ? token_weight[(long long)b * (T - 1) + t] : 1.f);
-    if (wsum) g /= wsum[b];
+    if (norm) g /= norm[b];
     const float l = lse[r];
     for (int c = threadIdx.x; c < nch; c += LOGP_THREADS) {
       float v[8];
@@ -1460,18 +1410,6 @@ extern "C" int rlaifv_f32_to_bf16_2d(const float* in, long long ld_in, void* out
   return 0;
 }
 
-extern "C" int rlaifv_logp_fwd(const void* logits, long long ld, const long long* labels, int nseq, int T, int V,
-                               float* per_tok, float* lse, float* logp_sum, float* logp_avg, float* count,
-                               void* stream) {
-  B200_REQUIRE(V % 8 == 0 && T >= 2, "logp_fwd: V %% 8 != 0 or T < 2");
-  const long long rows = (long long)nseq * (T - 1);
-  const int grid = (int)(rows < (long long)num_sms() * 8 ? rows : (long long)num_sms() * 8);
-  logp_fwd_kernel<<<grid, LOGP_THREADS, 0, ST>>>((const bf16*)logits, ld, labels, nseq, T, V, per_tok, lse, nullptr, 0);
-  B200_CHECK_CUDA(cudaGetLastError());
-  logp_reduce_kernel<<<nseq, 256, 0, ST>>>(per_tok, labels, nseq, T, logp_sum, logp_avg, count);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
 extern "C" int rlaifv_splice_token_weight(const int* src, const float* token_weight, float* out, int nseq, int Lw, int T,
                                           void* stream) {
   B200_REQUIRE(nseq > 0 && Lw > 0 && T >= 2, "splice_token_weight: bad shape");
@@ -1499,59 +1437,41 @@ extern "C" int rlaifv_rows_scatter(const int* row_pos, const void* dy, void* dx,
   B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
-// logits bf16 [n_rows][ld] = head applied to the gathered rows; per_tok [nseq][T-1] must be zero-filled by the caller
-// (unsupervised positions stay 0); lse fp32 [n_rows].
-extern "C" int rlaifv_logp_fwd_rows(const void* logits, long long ld, const long long* labels, const int* row_pos,
-                                    long long n_rows, int nseq, int T, int V, float* per_tok, float* lse,
-                                    float* logp_sum, float* logp_avg, float* count, void* stream) {
-  B200_REQUIRE(V % 8 == 0 && T >= 2 && n_rows > 0 && row_pos, "logp_fwd_rows: bad arguments");
-  const int grid = (int)(n_rows < (long long)num_sms() * 8 ? n_rows : (long long)num_sms() * 8);
+// row_pos NULL: dense logits [nseq*T][ld], lse [nseq][T]. Otherwise the compact rows: logits [n_rows][ld], lse
+// [n_rows], and per_tok [nseq][T-1] must be zero-filled by the caller (unsupervised positions stay 0).
+extern "C" int rlaifv_logp_fwd(const void* logits, long long ld, const long long* labels, const int* row_pos,
+                               long long n_rows, int nseq, int T, int V, float* per_tok, float* lse,
+                               float* logp_sum, float* logp_avg, float* count, void* stream) {
+  B200_REQUIRE(V % 8 == 0 && T >= 2, "logp_fwd: V %% 8 != 0 or T < 2");
+  B200_REQUIRE(!row_pos || n_rows > 0, "logp_fwd: n_rows <= 0 with row_pos");
+  const long long rows = row_pos ? n_rows : (long long)nseq * (T - 1);
+  const int grid = (int)(rows < (long long)num_sms() * 8 ? rows : (long long)num_sms() * 8);
   logp_fwd_kernel<<<grid, LOGP_THREADS, 0, ST>>>((const bf16*)logits, ld, labels, nseq, T, V, per_tok, lse, row_pos,
                                                  n_rows);
   B200_CHECK_CUDA(cudaGetLastError());
-  logp_reduce_kernel<<<nseq, 256, 0, ST>>>(per_tok, labels, nseq, T, logp_sum, logp_avg, count);
+  logp_reduce_kernel<<<nseq, 256, 0, ST>>>(per_tok, labels, nullptr, nseq, T, logp_sum, logp_avg, count);
   B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
-// in place on the compact logits: d loss / d logits. token_weight (nullable) [nseq][T-1]; norm (nullable) [nseq] =
-// label count (average mode) or weight sum (weighted average mode).
-extern "C" int rlaifv_logp_bwd_rows(void* logits, long long ld, const long long* labels, const int* row_pos,
-                                    long long n_rows, const float* lse, const float* d_logp, const float* token_weight,
-                                    const float* norm, int nseq, int T, int V, void* stream) {
-  B200_REQUIRE(V % 8 == 0 && n_rows > 0 && row_pos, "logp_bwd_rows: bad arguments");
-  const int grid = (int)(n_rows < (long long)num_sms() * 8 ? n_rows : (long long)num_sms() * 8);
-  logp_bwd_weighted_kernel<<<grid, LOGP_THREADS, 0, ST>>>((bf16*)logits, ld, labels, lse, d_logp, token_weight, norm,
-                                                          nseq, T, V, row_pos, n_rows);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-extern "C" int rlaifv_logp_bwd(void* logits, long long ld, const long long* labels, const float* lse,
-                               const float* d_logp, const float* count_or_null, int nseq, int T, int V,
-                               void* stream) {
+// in place: d loss / d logits, on the dense (row_pos NULL) or the compact logits. token_weight (nullable) [nseq][T-1];
+// norm (nullable) [nseq] = label count (average mode) or weight sum (weighted average mode).
+extern "C" int rlaifv_logp_bwd(void* logits, long long ld, const long long* labels, const int* row_pos,
+                               long long n_rows, const float* lse, const float* d_logp, const float* token_weight,
+                               const float* norm, int nseq, int T, int V, void* stream) {
   B200_REQUIRE(V % 8 == 0, "logp_bwd: V %% 8 != 0");
-  const long long rows = (long long)nseq * T;
+  B200_REQUIRE(!row_pos || n_rows > 0, "logp_bwd: n_rows <= 0 with row_pos");
+  const long long rows = row_pos ? n_rows : (long long)nseq * T;
   const int grid = (int)(rows < (long long)num_sms() * 8 ? rows : (long long)num_sms() * 8);
-  logp_bwd_kernel<<<grid, LOGP_THREADS, 0, ST>>>((bf16*)logits, ld, labels, lse, d_logp, count_or_null, nseq, T, V);
+  logp_bwd_kernel<<<grid, LOGP_THREADS, 0, ST>>>((bf16*)logits, ld, labels, lse, d_logp, token_weight, norm, nseq, T,
+                                                 V, row_pos, n_rows);
   B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
-
 extern "C" int rlaifv_logp_weighted_reduce(const float* per_tok, const long long* labels, const float* token_weight,
                                            int nseq, int T, float* logp_w, float* avg_w, float* wsum_or_null,
                                            void* stream) {
   B200_REQUIRE(nseq > 0 && T >= 2, "logp_weighted_reduce: bad shape");
-  logp_weighted_reduce_kernel<<<nseq, 256, 0, ST>>>(per_tok, labels, token_weight, nseq, T, logp_w, avg_w, wsum_or_null);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-extern "C" int rlaifv_logp_bwd_weighted(void* logits, long long ld, const long long* labels, const float* lse,
-                                        const float* d_logp, const float* token_weight, const float* wsum_or_null,
-                                        int nseq, int T, int V, void* stream) {
-  B200_REQUIRE(V % 8 == 0 && token_weight != nullptr, "logp_bwd_weighted: V %% 8 != 0 or no weights");
-  const long long rows = (long long)nseq * T;
-  const int grid = (int)(rows < (long long)num_sms() * 8 ? rows : (long long)num_sms() * 8);
-  logp_bwd_weighted_kernel<<<grid, LOGP_THREADS, 0, ST>>>((bf16*)logits, ld, labels, lse, d_logp, token_weight,
-                                                          wsum_or_null, nseq, T, V, nullptr, 0);
+  logp_reduce_kernel<<<nseq, 256, 0, ST>>>(per_tok, labels, token_weight, nseq, T, logp_w, avg_w, wsum_or_null);
   B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -64,14 +64,10 @@ _SIGNATURES = {
     "rlaifv_supervised_rows": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
     "rlaifv_rows_gather": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
     "rlaifv_rows_scatter": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
-    "rlaifv_logp_fwd_rows": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                             c_void_p, c_void_p, c_void_p],
-    "rlaifv_logp_bwd_rows": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                             c_int, c_int, c_void_p],
-    "rlaifv_logp_fwd": [c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+    "rlaifv_logp_fwd": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                         c_void_p, c_void_p, c_void_p],
-    "rlaifv_logp_bwd": [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                        c_void_p],
+    "rlaifv_logp_bwd": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                        c_int, c_int, c_void_p],
     "rlaifv_dpo_loss": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_float, c_float, c_float,
                         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "rlaifv_adamw_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_ll, c_float, c_float,
@@ -100,8 +96,6 @@ _SIGNATURES = {
                              c_int, c_float, c_void_p],
     "rlaifv_add_rows_bcast": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
     "rlaifv_logp_weighted_reduce": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
-    "rlaifv_logp_bwd_weighted": [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                 c_void_p],
     "rlaifv_splice_map_inplace": [c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_void_p, c_void_p,
                                   c_void_p],
 }

@@ -641,31 +641,25 @@ class LlavaDPOPolicy:
         self._need("embed")
         x, new_labels, src, T = self.splice(input_ids, labels, proj, b, img_index,
                                             T_hint=(T_hint, n_slots) if T_hint is not None else None)
-        M = nseq * T
         if keep_stash:
             st.update(src=src, input_ids=input_ids, labels=new_labels, T=T, nseq=nseq, b=b,
                       n_feat_rows=proj.shape[0])
         x = self._run_layers(x, nseq, T, st)
         self._need("head")
         compact = keep_stash and self.compact_head
+        row_pos = None
         if compact:
             # training: only the positions whose next token is supervised reach the final norm / lm_head / log-softmax
             # (get_batch_logps masks the rest out of the sum, muffin_inference_logp.py:93-104). A row of the collator
             # holds at most L labels, so L slots per sequence always suffice — no host sync for the count.
             row_pos = ops.supervised_rows(new_labels, input_ids.shape[1])
-            R = row_pos.numel()
-            xc = ops.rows_gather(row_pos, x, out=self.buf("xc", (R, H)))
-            rstd_f = torch.empty(R, dtype=_F32, device=dev)
-            hn = ops.rmsnorm_fwd(xc, P["norm"], d.rms_eps, out=self.buf("hn_c", (R, H)), rstd=rstd_f)
-            logits = ops.gemm(hn, P["lm_head"], self.buf("logits_c", (R, V)))
-            per_tok, lse_v, logp, avg, count = ops.logp_fwd_rows(logits, new_labels, row_pos, nseq, T)
-            st.update(x_final=xc, rstd_f=rstd_f, hn=hn, logits=logits, lse_v=lse_v, count=count, row_pos=row_pos)
-            self._stash = st
-            return dict(per_token_logps=per_tok, logp=logp, avg_logp=avg, labels=new_labels, T=T)
-        rstd_f = torch.empty(M, dtype=_F32, device=dev) if keep_stash else None
-        hn = ops.rmsnorm_fwd(x, P["norm"], d.rms_eps, out=self.buf("hn", (M, H)), rstd=rstd_f)
-        logits = ops.gemm(hn, P["lm_head"], self.buf("logits", (M, V)))
-        per_tok, lse_v, logp, avg, count = ops.logp_fwd(logits, new_labels, nseq, T)
+            x = ops.rows_gather(row_pos, x, out=self.buf("xc", (row_pos.numel(), H)))
+            st["row_pos"] = row_pos
+        R, sfx = x.shape[0], "_c" if compact else ""      # rows that reach the head (M, or the compact row count)
+        rstd_f = torch.empty(R, dtype=_F32, device=dev) if keep_stash else None
+        hn = ops.rmsnorm_fwd(x, P["norm"], d.rms_eps, out=self.buf("hn" + sfx, (R, H)), rstd=rstd_f)
+        logits = ops.gemm(hn, P["lm_head"], self.buf("logits" + sfx, (R, V)))
+        per_tok, lse_v, logp, avg, count = ops.logp_fwd(logits, new_labels, nseq, T, row_pos=row_pos)
         if keep_stash:
             st.update(x_final=x, rstd_f=rstd_f, hn=hn, logits=logits, lse_v=lse_v, count=count)
             self._stash = st
@@ -688,19 +682,12 @@ class LlavaDPOPolicy:
         cos, sin = self.rope_tables(T)
         acc = bool(accumulate)
 
-        row_pos = st.get("row_pos")
+        row_pos = st.get("row_pos")               # compact head (training): logits hold the supervised rows only
         if token_weight is not None:
             assert not use_average or weight_sum is not None
-        if row_pos is not None:                   # compact head (training): logits hold the supervised rows only
-            norm = (weight_sum if token_weight is not None else st["count"]) if use_average else None
-            dlogits = ops.logp_bwd_rows(st["logits"], st["labels"], row_pos, st["lse_v"], d_logp, nseq, T,
-                                        token_weight=token_weight, norm=norm)
-        elif token_weight is not None:
-            dlogits = ops.logp_bwd_weighted(st["logits"], st["labels"], st["lse_v"], d_logp, token_weight, nseq, T,
-                                            wsum=weight_sum if use_average else None)
-        else:
-            dlogits = ops.logp_bwd(st["logits"], st["labels"], st["lse_v"], d_logp, nseq, T,
-                                   count=st["count"] if use_average else None)
+        norm = (weight_sum if token_weight is not None else st["count"]) if use_average else None
+        dlogits = ops.logp_bwd(st["logits"], st["labels"], st["lse_v"], d_logp, nseq, T, row_pos=row_pos,
+                               token_weight=token_weight, norm=norm)
         frozen = self.lora is not None            # LoRA: lm_head / norms / embeddings / base matrices are frozen
         scratch_h = self.buf("frozen_dw", (H,)) if frozen else None
         Mh = dlogits.shape[0]                     # rows that went through the head (M, or the compact row count)

@@ -362,20 +362,25 @@ def f32_to_bf16_2d(src, dst, accumulate=False):
     return dst
 
 
-def logp_fwd(logits, labels, nseq, T):
-    """logits [nseq*T, V] bf16 (row stride may exceed V); labels [nseq, T] int64 (spliced).
-    Returns per_tok [nseq, T-1], lse [nseq, T], logp_sum, logp_avg, count [nseq] (all fp32)."""
+def logp_fwd(logits, labels, nseq, T, row_pos=None):
+    """logits [nseq*T, V] bf16 (row stride may exceed V), or with row_pos (compact head) [n_rows, V] of the gathered
+    rows; labels [nseq, T] int64 (spliced). Returns per_tok [nseq, T-1] (zeros at unsupervised positions when compact),
+    lse [nseq, T] (compact: [n_rows]), logp_sum, logp_avg, count [nseq] (all fp32)."""
     _chk(logits)
     assert labels.dtype == torch.int64 and labels.is_contiguous()
-    V = logits.shape[1]
-    dev = logits.device
-    per_tok = torch.empty((nseq, T - 1), dtype=_f32, device=dev)
-    lse = torch.zeros((nseq, T), dtype=_f32, device=dev)
+    (n, V), dev = logits.shape, logits.device
+    if row_pos is None:
+        per_tok = torch.empty((nseq, T - 1), dtype=_f32, device=dev)
+        lse = torch.zeros((nseq, T), dtype=_f32, device=dev)
+    else:
+        assert row_pos.numel() == n
+        per_tok = torch.zeros((nseq, T - 1), dtype=_f32, device=dev)
+        lse = torch.zeros(n, dtype=_f32, device=dev)
     s = torch.empty(nseq, dtype=_f32, device=dev)
     a = torch.empty(nseq, dtype=_f32, device=dev)
     c = torch.empty(nseq, dtype=_f32, device=dev)
-    _l.call("rlaifv_logp_fwd", _l.ptr(logits), logits.stride(0), _l.ptr(labels), nseq, T, V, _l.ptr(per_tok),
-            _l.ptr(lse), _l.ptr(s), _l.ptr(a), _l.ptr(c), _l.stream_ptr())
+    _l.call("rlaifv_logp_fwd", _l.ptr(logits), logits.stride(0), _l.ptr(labels), _l.ptr(row_pos), n, nseq, T, V,
+            _l.ptr(per_tok), _l.ptr(lse), _l.ptr(s), _l.ptr(a), _l.ptr(c), _l.stream_ptr())
     return per_tok, lse, s, a, c
 
 
@@ -418,35 +423,16 @@ def rows_scatter(row_pos, dy, dx):
     return dx
 
 
-def logp_fwd_rows(logits, labels, row_pos, nseq, T):
-    """Compact-head form of logp_fwd: logits [n_rows, V] of the gathered rows. Returns per_tok [nseq, T-1] (zeros at
-    unsupervised positions), lse [n_rows], logp_sum, logp_avg, count."""
-    _chk(logits)
-    V, dev, n = logits.shape[1], logits.device, row_pos.numel()
-    assert logits.shape[0] == n
-    per_tok = torch.zeros((nseq, T - 1), dtype=_f32, device=dev)
-    lse = torch.zeros(n, dtype=_f32, device=dev)
-    s = torch.empty(nseq, dtype=_f32, device=dev)
-    a = torch.empty(nseq, dtype=_f32, device=dev)
-    c = torch.empty(nseq, dtype=_f32, device=dev)
-    _l.call("rlaifv_logp_fwd_rows", _l.ptr(logits), logits.stride(0), _l.ptr(labels), _l.ptr(row_pos), n, nseq, T, V,
-            _l.ptr(per_tok), _l.ptr(lse), _l.ptr(s), _l.ptr(a), _l.ptr(c), _l.stream_ptr())
-    return per_tok, lse, s, a, c
-
-
-def logp_bwd_rows(logits, labels, row_pos, lse, d_logp, nseq, T, token_weight=None, norm=None):
-    """In place on the compact logits: logits <- d loss / d logits (token_weight [nseq, T-1] / norm [nseq] optional)."""
+def logp_bwd(logits, labels, lse, d_logp, nseq, T, row_pos=None, token_weight=None, norm=None):
+    """In place on the dense or (row_pos given) compact logits: logits <- d loss / d logits. token_weight [nseq, T-1]:
+    token-weighted log-prob; norm [nseq] (average mode): the label count, or the weight sum when weighted."""
     _chk(logits), _chk(lse, _f32), _chk(d_logp, _f32)
-    _l.call("rlaifv_logp_bwd_rows", _l.ptr(logits), logits.stride(0), _l.ptr(labels), _l.ptr(row_pos), row_pos.numel(),
+    assert row_pos is None or row_pos.numel() == logits.shape[0]
+    if token_weight is not None:
+        _chk(token_weight, _f32)
+        assert tuple(token_weight.shape) == (nseq, T - 1) and token_weight.is_contiguous()
+    _l.call("rlaifv_logp_bwd", _l.ptr(logits), logits.stride(0), _l.ptr(labels), _l.ptr(row_pos), logits.shape[0],
             _l.ptr(lse), _l.ptr(d_logp), _l.ptr(token_weight), _l.ptr(norm), nseq, T, logits.shape[1], _l.stream_ptr())
-    return logits
-
-
-def logp_bwd(logits, labels, lse, d_logp, nseq, T, count=None):
-    """In place: logits <- d loss / d logits."""
-    _chk(logits), _chk(lse, _f32), _chk(d_logp, _f32)
-    _l.call("rlaifv_logp_bwd", _l.ptr(logits), logits.stride(0), _l.ptr(labels), _l.ptr(lse), _l.ptr(d_logp),
-            _l.ptr(count), nseq, T, logits.shape[1], _l.stream_ptr())
     return logits
 
 
@@ -463,15 +449,6 @@ def logp_weighted_reduce(per_tok, labels, token_weight):
     _l.call("rlaifv_logp_weighted_reduce", _l.ptr(per_tok), _l.ptr(labels), _l.ptr(token_weight), nseq, T, _l.ptr(lw),
             _l.ptr(aw), _l.ptr(ws), _l.stream_ptr())
     return lw, aw, ws
-
-
-def logp_bwd_weighted(logits, labels, lse, d_logp, token_weight, nseq, T, wsum=None):
-    """In place: logits <- d loss / d logits for the token-weighted log-prob (wsum given = average mode)."""
-    _chk(logits), _chk(lse, _f32), _chk(d_logp, _f32), _chk(token_weight, _f32)
-    assert tuple(token_weight.shape) == (nseq, T - 1) and token_weight.is_contiguous()
-    _l.call("rlaifv_logp_bwd_weighted", _l.ptr(logits), logits.stride(0), _l.ptr(labels), _l.ptr(lse), _l.ptr(d_logp),
-            _l.ptr(token_weight), _l.ptr(wsum), nseq, T, logits.shape[1], _l.stream_ptr())
-    return logits
 
 
 def dpo_loss(policy_win, policy_rej, ref_win, ref_rej, beta, dpo_weight=1.0, sft_weight=0.0, grad_scale=1.0,

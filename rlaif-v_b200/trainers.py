@@ -83,8 +83,8 @@ def dpo_loss(policy_chosen_logps, policy_rejected_logps, reference_chosen_logps,
 def compute_weighted_logp(per_token_logp, labels, token_weight, use_average):
     """muffin/train/trainers.py:128-137, for host-side tensors (the frozen-reference per-token log-probs the collator
     delivers). The policy side of the token-weighted loss runs in the CUDA library (ops.logp_weighted_reduce /
-    ops.logp_bwd_weighted through DPOStepEngine(dpo_token_weighted=True)); the reference — and this drop-in — raise
-    NotImplementedError for LLaVA-1.5 (:246-248), the branch exists for the OmniLMM / MiniCPM-style models."""
+    ops.logp_bwd(token_weight=...) through DPOStepEngine(dpo_token_weighted=True)); the reference — and this drop-in —
+    raise NotImplementedError for LLaVA-1.5 (:246-248), the branch exists for the OmniLMM / MiniCPM-style models."""
     loss_mask = labels[:, 1:] != -100
     weighted_mask = token_weight * loss_mask
     logp = (per_token_logp * weighted_mask).sum(-1)

@@ -8,9 +8,16 @@ import torch
 
 from oracle import llava_dpo_oracle as O
 
+# argument positions of rlaifv_logp_fwd / rlaifv_logp_bwd (include/rlaifv_b200.h)
+ROW_POS, TOKEN_WEIGHT = 3, 7
+
+
+def _nonnull(p):
+    return p.value is not None      # ops passes None as c_void_p(0), whose value is None
+
 
 @pytest.mark.parametrize("use_lora,cfg_name", [(False, "TINY"), (True, "TINY"), (False, "TINY_GQA")])
-def test_launch_sequence_dry_run(monkeypatch, use_lora, cfg_name):
+def test_launch_sequence_and_head_arguments_dry_run(monkeypatch, use_lora, cfg_name):
     from rlaifv_b200 import lib, ops
     from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
     c = O.CONFIGS[cfg_name]
@@ -19,11 +26,12 @@ def test_launch_sequence_dry_run(monkeypatch, use_lora, cfg_name):
                      clip_hidden=c.clip_hidden,
                      clip_intermediate=c.clip_intermediate, clip_layers=c.clip_layers, clip_heads=c.clip_heads,
                      image_size=c.image_size, patch_size=c.patch_size)
-    calls = []
+    calls, argv = [], {}
 
     def fake_call(name, *args):
         assert len(args) == len(lib._SIGNATURES[name]), name       # argument count matches the ctypes table
         calls.append(name)
+        argv.setdefault(name, []).append(args)
 
     monkeypatch.setattr(lib, "call", fake_call)
     monkeypatch.setattr(lib, "stream_ptr", lambda: ctypes.c_void_p(0))
@@ -59,10 +67,13 @@ def test_launch_sequence_dry_run(monkeypatch, use_lora, cfg_name):
     assert calls.count("rlaifv_attention_fwd") + calls.count("rlaifv_attention_fwd_gqa") == \
         dims.num_layers + dims.clip_layers_used
     assert calls.count("rlaifv_attention_fwd_gqa") == (dims.num_layers if gqa else 0)
-    # decoder backward: the split dK/dV + dQ kernels (one C-ABI entry for MHA and GQA), compact-head log-prob rows
+    # decoder backward: the split dK/dV + dQ kernels (one C-ABI entry for MHA and GQA)
     assert calls.count("rlaifv_attention_bwd_split") == dims.num_layers
-    assert calls.count("rlaifv_supervised_rows") == 1 and calls.count("rlaifv_logp_fwd_rows") == 1
-    assert calls.count("rlaifv_logp_bwd_rows") == 1 and calls.count("rlaifv_rows_scatter") == 1
+    # compact head: the log-prob forward and backward run on the rows supervised_rows picked
+    assert calls.count("rlaifv_supervised_rows") == 1 and calls.count("rlaifv_rows_scatter") == 1
+    (rows,), (fwd,), (bwd,) = argv["rlaifv_supervised_rows"], argv["rlaifv_logp_fwd"], argv["rlaifv_logp_bwd"]
+    assert _nonnull(fwd[ROW_POS]) and fwd[ROW_POS].value == bwd[ROW_POS].value == rows[4].value
+    assert not _nonnull(bwd[TOKEN_WEIGHT])
     names = {b.name for b in pol.trainable_buckets()}
     assert ("projector" in names) and (("lora0" in names) == use_lora) and (("embed" in names) != use_lora)
 
@@ -97,18 +108,19 @@ def test_resampler_launch_sequence_dry_run(monkeypatch):
     assert torch.allclose(m.pos_embed_f32, R.sincos_2d(c.embed_dim, c.grid_size), atol=1e-6)
 
 
-def test_omnilmm_policy_launch_sequence_dry_run(monkeypatch):
+def test_omnilmm_policy_launch_sequence_and_head_arguments_dry_run(monkeypatch):
     """OmniLMM policy (resampler front-end + in-place splice + GQA decoder) against the recording C ABI; also runs the
     bf16 oracle path once so the GPU parity test's CPU half is known to work."""
     from rlaifv_b200 import lib, ops
     from rlaifv_b200.model import LlavaDims
     from rlaifv_b200.omnilmm_model import OmniLMMDPOPolicy, omnilmm_dims
     from oracle import omnilmm_oracle as OM
-    calls = []
+    calls, argv = [], {}
 
     def fake_call(name, *args):
         assert len(args) == len(lib._SIGNATURES[name]), name
         calls.append(name)
+        argv.setdefault(name, []).append(args)
 
     monkeypatch.setattr(lib, "call", fake_call)
     monkeypatch.setattr(lib, "stream_ptr", lambda: ctypes.c_void_p(0))
@@ -135,14 +147,15 @@ def test_omnilmm_policy_launch_sequence_dry_run(monkeypatch):
     assert calls.count("rlaifv_splice_map_inplace") == 1 and calls.count("rlaifv_cross_attention_bwd") == 1
     assert calls.count("rlaifv_attention_fwd_gqa") == d.num_layers and "rlaifv_clip_im2col" not in calls
     assert pol.vision_token_grad.shape == batch["vision_tokens"].shape
-    # token-weighted variant (--dpo_token_weighted): weighted reduce + weighted backward entry points
+    # token-weighted variant (--dpo_token_weighted): weighted reduce + the backward with token weights
     out = pol.forward_logps(batch["concatenated_input_ids"], batch["concatenated_labels"], batch["vision_tokens"])
     tw = torch.ones(4, L - 1)
     lw, aw, ws = ops.logp_weighted_reduce(out["per_token_logps"], out["labels"], tw)
-    n_rows = calls.count("rlaifv_logp_bwd_rows")
     pol.backward_logps(torch.zeros(4), use_average=True, token_weight=tw, weight_sum=ws)
-    # compact head: the weighted and the plain backward share the rows entry point (token_weight / norm arguments)
-    assert calls.count("rlaifv_logp_bwd_rows") == n_rows + 1 and calls.count("rlaifv_logp_bwd") == 0
+    # compact head: the weighted and the plain backward share one entry point (token_weight / norm arguments)
+    fwds, bwds = argv["rlaifv_logp_fwd"], argv["rlaifv_logp_bwd"]
+    assert len(fwds) == len(bwds) == 2 and all(_nonnull(a[ROW_POS]) for a in fwds + bwds)
+    assert not _nonnull(bwds[0][TOKEN_WEIGHT]) and _nonnull(bwds[1][TOKEN_WEIGHT])
     # generic get_beta_and_logps branch (forward_DPO) incl. --dpo_token_weighted, autograd bridge end to end
     from types import SimpleNamespace
     from rlaifv_b200 import trainers
@@ -155,12 +168,14 @@ def test_omnilmm_policy_launch_sequence_dry_run(monkeypatch):
               "ref_rej_logp": torch.zeros(2), "beta": 0.1, "images": batch["vision_tokens"],
               "concatenated_input_ids": ids, "concatenated_labels": labels, "concatenated_attention_mask": None}
         args = SimpleNamespace(dpo_use_average=False, dpo_token_weighted=weighted, task="DPO")
-        n_w = calls.count("rlaifv_logp_bwd_rows")
+        n_w = len(argv["rlaifv_logp_bwd"])
         pw, pr, rw, rr, beta = trainers.get_beta_and_logps(dd, pol, args, is_llava15=False)
         assert pw.shape == (2,) and pr.shape == (2,) and pw.requires_grad and not dd
         losses, cr, rj = trainers.dpo_loss(pw, pr, rw, rr, beta)
         losses.mean().backward()
-        assert calls.count("rlaifv_logp_bwd_rows") == n_w + 1
+        assert len(argv["rlaifv_logp_bwd"]) == n_w + 1
+        bwd = argv["rlaifv_logp_bwd"][-1]
+        assert _nonnull(bwd[ROW_POS]) and _nonnull(bwd[TOKEN_WEIGHT]) == weighted
     with pytest.raises(ValueError):
         trainers.get_beta_and_logps({**{k: None for k in ("win_input_ids", "rej_input_ids", "ref_win_avg_logp",
                                                           "ref_rej_avg_logp", "ref_win_logp", "ref_rej_logp", "beta",

@@ -137,8 +137,8 @@ def test_omnilmm_engine_step_trains_decoder_and_resampler():
     assert float(m2[0]) < loss1                             # one AdamW step on the same batch lowers the loss
 
 
-def test_weighted_logp_kernels_match_torch():
-    """rlaifv_logp_weighted_reduce / rlaifv_logp_bwd_weighted vs fp32 torch (sum and average mode)."""
+def test_weighted_logp_reduce_and_backward_match_torch():
+    """rlaifv_logp_weighted_reduce / rlaifv_logp_bwd with token weights vs fp32 torch (sum and average mode)."""
     from rlaifv_b200 import ops
     g = torch.Generator().manual_seed(2)
     nseq, T, V = 3, 37, 320
@@ -159,7 +159,7 @@ def test_weighted_logp_kernels_match_torch():
         lw, aw, ws = ops.logp_weighted_reduce(per_tok, labels.cuda(), tw.cuda())
         got = (aw if use_avg else lw).cpu()
         assert rel(got, ref.detach()) < 2e-3
-        ops.logp_bwd_weighted(lg, labels.cuda(), lse, d.cuda(), tw.cuda(), nseq, T, wsum=ws if use_avg else None)
+        ops.logp_bwd(lg, labels.cuda(), lse, d.cuda(), nseq, T, token_weight=tw.cuda(), norm=ws if use_avg else None)
         torch.cuda.synchronize()
         want = lf.grad.view(nseq * T, V)
         assert float((lg.float().cpu() - want).norm() / want.norm()) < 8e-3
