@@ -144,6 +144,34 @@ int rlaifv_rope_fwd_gqa(void* qkv, const void* cos_tab, const void* sin_tab, lon
 int rlaifv_rope_bwd_gqa(void* dqkv, const float* dq_f32, const void* cos_tab, const void* sin_tab, long long M,
                         int T, int n_heads, int n_kv_heads, int head_dim, long long ld, void* stream);
 
+/* ---- packed rows: variable-length causal decoder (DESIGN.md §3) ---------------------------------
+ * A training batch may drop every row after its sequence's last supervised position: sequence s then occupies rows
+ * [cu[s], cu[s+1]) of [n_rows][ld] buffers, row cu[s] + t being position t. cu is int32 [nseq + 1] on the device;
+ * max_len >= the longest sequence (sizes the grid). lse and delta_ws are fp32 [n_heads * n_rows], sequence s's
+ * [n_heads][len_s] block at offset n_heads * cu[s]. Causal, head_dim 128, n_kv_heads <= n_heads (GQA). Every valid
+ * row gets the bits the fixed-length kernels give the same sequence padded. The backward is the split form: dq bf16
+ * [n_rows][ld_dq] (may be the q block of a fused dqkv buffer), dk/dv bf16 [n_rows][ld_dkv]. */
+int rlaifv_attention_varlen_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out,
+                                long long ld_out, float* lse, const int* cu, int nseq, int max_len, long long n_rows,
+                                int n_heads, int n_kv_heads, int head_dim, float scale, void* stream);
+int rlaifv_attention_varlen_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out,
+                                long long ld_out, const void* d_out, long long ld_dout, const float* lse, void* dq,
+                                long long ld_dq, void* dk, void* dv, long long ld_dkv, float* delta_ws, const int* cu,
+                                int nseq, int max_len, long long n_rows, int n_heads, int n_kv_heads, int head_dim,
+                                float scale, void* stream);
+/* RoPE on the fused [q | k | v] rows with the position of row m taken from pos[m] (int32 [M], device); the backward
+ * rotates the q block (split attention backward) and the k block in place. */
+int rlaifv_rope_pos_fwd(void* qkv, const void* cos_tab, const void* sin_tab, const int* pos, long long M, int n_heads,
+                        int n_kv_heads, int head_dim, long long ld, void* stream);
+int rlaifv_rope_pos_bwd(void* dqkv, const void* cos_tab, const void* sin_tab, const int* pos, long long M, int n_heads,
+                        int n_kv_heads, int head_dim, long long ld, void* stream);
+/* LoRA dropout on packed rows x [n_rows][width]: row r draws the keep bits of row rows[r] of rlaifv_dropout_fwd's
+ * element order, so a packed step draws the padded step's masks. */
+int rlaifv_dropout_rows_fwd(const void* x, void* out, const int* rows, long long n_rows, int width, float p,
+                            unsigned long long seed, void* stream);
+int rlaifv_dropout_rows_bwd_add(void* dx, const void* g, const int* rows, long long n_rows, int width, float p,
+                                unsigned long long seed, void* stream);
+
 /* ---- norms (HF:llama/modeling_llama.py:62-67; HF:clip LayerNorm) -------------------------------- */
 int rlaifv_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd_or_null, int M, int H, float eps,
                        void* stream);

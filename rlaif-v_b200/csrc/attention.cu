@@ -763,3 +763,554 @@ extern "C" int rlaifv_cross_attention_bwd(const void* q, long long ld_q, const v
   return attention_bwd_impl(q, ld_q, k, v, ld_kv, out, ld_out, d_out, ld_dout, lse, nullptr, 0, dq_f32, dk, dv, ld_dkv, delta_ws,
                             nseq, Sq, Skv, n_heads, n_heads, head_dim, 0, q_shared, scale, stream);
 }
+
+// ================================================================================================
+// variable-length causal self-attention over packed rows (head_dim 128, MHA or GQA)
+// ================================================================================================
+// Sequence s occupies rows [cu[s], cu[s+1]) of q/k/v/out [n_rows][ld]; its row cu[s] + t is position t. LSE and the
+// delta workspace are fp32 with sequence s's [n_heads][len_s] block at offset n_heads * cu[s]. Tiles are cut relative
+// to cu[s], so every valid row sees the key partition, online-softmax order and chunk order of the fixed-length
+// kernels above on the same sequence padded to any length: the results at rows < len_s are the same bits. A tile's
+// rows past len_s are the next sequence's (or TMA zero-fill past the last row): causality hides them from valid
+// queries in the forward and the dQ kernel; the dK/dV kernel, where they come after the key, masks them explicitly.
+namespace b200 {
+
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_varlen_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                            const __grid_constant__ CUtensorMap tmV, bf16* __restrict__ out, long long ld_out,
+                            float* __restrict__ lse_out, const int* __restrict__ cu, int n_heads, int kv_group,
+                            float scale) {
+  constexpr int D = 128;
+  using Cfg = AttFwdCfg<D>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;                 // [STAGES]
+  uint64_t* kv_empty = bars + 1 + ATT_STAGES;   // [STAGES]
+
+  const int seq = blockIdx.z;
+  const int row0 = cu[seq], len = cu[seq + 1] - row0;
+  const int num_q_tiles = (len + ATT_BQ - 1) / ATT_BQ;
+  if ((int)blockIdx.x >= num_q_tiles) return;             // the grid is sized for the longest sequence
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const int q_tile = num_q_tiles - 1 - blockIdx.x;        // heavy (late) tiles first
+  const int head = blockIdx.y;
+  const int kv_head = head / kv_group;
+  const int q0 = q_tile * ATT_BQ;
+  const int n_kv = min(num_q_tiles, (q0 + ATT_BQ + ATT_BKV - 1) / ATT_BKV);
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int i = 0; i < ATT_STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    if (threadIdx.x == 256) {
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmK);
+      tma_prefetch_desc(&tmV);
+      mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
+#pragma unroll
+      for (int a = 0; a < D / 64; ++a) tma_load_2d(smem + a * Cfg::Q_ATOM, &tmQ, q_full, head * D + a * 64, row0 + q0);
+      for (int j = 0; j < n_kv; ++j) {
+        const int s = j % ATT_STAGES;
+        if (j >= ATT_STAGES) mbar_wait(&kv_empty[s], ((j / ATT_STAGES) - 1) & 1);
+        mbar_arrive_expect_tx(&kv_full[s], 2 * Cfg::KV_BYTES);
+#pragma unroll
+        for (int a = 0; a < D / 64; ++a) {
+          tma_load_2d(smem + Cfg::OFF_K + s * Cfg::KV_BYTES + a * Cfg::KV_ATOM, &tmK, &kv_full[s],
+                      kv_head * D + a * 64, row0 + j * ATT_BKV);
+          tma_load_2d(smem + Cfg::OFF_V + s * Cfg::KV_BYTES + a * Cfg::KV_ATOM, &tmV, &kv_full[s],
+                      kv_head * D + a * 64, row0 + j * ATT_BKV);
+        }
+      }
+    }
+  } else {
+    const FragPos fp = frag_pos();
+    const int qr[2] = {q0 + wg * 64 + fp.r0, q0 + wg * 64 + fp.r0 + 8};
+    const float c = scale * LOG2E;
+    float o[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    const uint32_t q_addr = smem_u32(smem) + wg * 64 * 128;
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < n_kv; ++j) {
+      const int s = j % ATT_STAGES;
+      mbar_wait(&kv_full[s], (j / ATT_STAGES) & 1);
+      const uint32_t k_addr = smem_u32(smem + Cfg::OFF_K + s * Cfg::KV_BYTES);
+      const uint32_t v_addr = smem_u32(smem + Cfg::OFF_V + s * Cfg::KV_BYTES);
+      float sv[64];
+      wgmma_fence();
+      mma_qk_128<D>(sv, q_addr, Cfg::Q_ATOM, k_addr, Cfg::KV_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(sv);
+      const int kv0 = j * ATT_BKV;
+      if (kv0 + ATT_BKV > len || kv0 + ATT_BKV - 1 > q0 + wg * 64) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int kv = kv0 + 8 * i + fp.c0 + (e & 1);
+            if (kv >= len || kv > qr[e >> 1]) sv[4 * i + e] = -INFINITY;
+          }
+      }
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        mx[0] = fmaxf(mx[0], fmaxf(sv[4 * i], sv[4 * i + 1]));
+        mx[1] = fmaxf(mx[1], fmaxf(sv[4 * i + 2], sv[4 * i + 3]));
+      }
+      float alpha[2], neg_m[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        float m_new = fmaxf(m_run[h], mx[h] * c);
+        if (m_new == -INFINITY) m_new = 0.f;
+        if (j > 0 && m_new - m_run[h] <= 8.0f) m_new = m_run[h];   // lazy max, as attention_fwd_kernel
+        alpha[h] = fast_exp2(m_run[h] - m_new);
+        m_run[h] = m_new;
+        l[h] *= alpha[h];
+        neg_m[h] = -m_new;
+      }
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i) {
+        o[4 * i] *= alpha[0]; o[4 * i + 1] *= alpha[0];
+        o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
+      }
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float p = fast_exp2(fmaf(sv[4 * i + e], c, neg_m[e >> 1]));
+          sv[4 * i + e] = p;
+          l[e >> 1] += p;
+        }
+      uint32_t pa[8][4];
+      acc_to_afrag<8>(sv, pa);
+      reg_fence(o);
+      wgmma_fence();
+      mma_pv<D, 8>(o, pa, v_addr, Cfg::KV_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
+      if (lane == 0) mbar_arrive(&kv_empty[s]);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+      const int q = qr[h];
+      if (q >= len) continue;
+      const float inv = 1.f / l[h];
+      bf16* o_row = out + ((long long)row0 + q) * ld_out + head * D + fp.c0;
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i)
+        *reinterpret_cast<uint32_t*>(o_row + 8 * i) = pack_bf16(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+      if (fp.c0 == 0) lse_out[(long long)n_heads * row0 + (long long)head * len + q] = (m_run[h] + log2f(l[h])) * LN2;
+    }
+  }
+}
+
+// delta of attention_delta_kernel over packed rows, stored in the packed [n_heads][len_s] blocks
+__global__ void attention_varlen_delta_kernel(const bf16* __restrict__ o, long long ld_o, const bf16* __restrict__ d_o,
+                                              long long ld_do, float* __restrict__ delta, const int* __restrict__ cu,
+                                              int nseq, long long n_rows, int n_heads, int D) {
+  const int lpi = D >> 3;
+  const int ipw = 32 / lpi;
+  const long long total = n_rows * n_heads;
+  const int wpb = blockDim.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int sub = lane / lpi, l = lane % lpi;
+  const long long stride = (long long)gridDim.x * wpb * ipw * 2;
+  for (long long base = ((long long)blockIdx.x * wpb + (threadIdx.x >> 5)) * ipw * 2; base < total; base += stride) {
+    float acc[2];
+    long long item[2];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      item[u] = base + u * ipw + sub;
+      acc[u] = 0.f;
+      if (item[u] < total) {
+        const int head = (int)(item[u] % n_heads);
+        const long long row = item[u] / n_heads;
+        const uint4 a = *reinterpret_cast<const uint4*>(o + row * ld_o + head * D + l * 8);
+        const uint4 b = *reinterpret_cast<const uint4*>(d_o + row * ld_do + head * D + l * 8);
+        const float2 a0 = unpack_bf16(a.x), a1 = unpack_bf16(a.y), a2 = unpack_bf16(a.z), a3 = unpack_bf16(a.w);
+        const float2 b0 = unpack_bf16(b.x), b1 = unpack_bf16(b.y), b2 = unpack_bf16(b.z), b3 = unpack_bf16(b.w);
+        acc[u] = a0.x * b0.x + a0.y * b0.y + a1.x * b1.x + a1.y * b1.y + a2.x * b2.x + a2.y * b2.y + a3.x * b3.x +
+                 a3.y * b3.y;
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      for (int off = lpi >> 1; off > 0; off >>= 1) acc[u] += __shfl_xor_sync(0xffffffffu, acc[u], off);
+      if (l == 0 && item[u] < total) {
+        const int head = (int)(item[u] % n_heads);
+        const int row = (int)(item[u] / n_heads);
+        int lo = 0, hi = nseq - 1;                             // sequence s with cu[s] <= row < cu[s + 1]
+        while (lo < hi) {
+          const int mid = (lo + hi + 1) >> 1;
+          if (cu[mid] <= row) lo = mid; else hi = mid - 1;
+        }
+        const int row0 = cu[lo], len = cu[lo + 1] - row0;
+        delta[(long long)n_heads * row0 + (long long)head * len + (row - row0)] = acc[u];
+      }
+    }
+  }
+}
+
+// one pass of attention_bwd_dkv_kernel over packed rows; query rows >= len are masked (P = dS = 0)
+template <bool DK>
+__device__ __forceinline__ void varlen_dkv_pass(uint8_t* smem, uint64_t* c_full, uint64_t* c_empty, int it0, int n_it,
+                                                int n_c, int c_first, int kv_head, int kv_group, long long blk0, int len,
+                                                const int (&kvr)[2], uint32_t k_addr, uint32_t v_addr, float c,
+                                                float scale, const float* __restrict__ lse,
+                                                const float* __restrict__ delta, float (&acc)[BWD_D / 2]) {
+  using Cfg = AttBwdCfg;
+  const FragPos fp = frag_pos();
+#pragma unroll
+  for (int i = 0; i < BWD_D / 2; ++i) acc[i] = 0.f;
+  for (int it = 0; it < n_it; ++it) {
+    const int ii = it0 + it, s = ii % ATT_STAGES;
+    const int qc0 = (c_first + it % n_c) * BWD_C;
+    const int head = kv_head * kv_group + it / n_c;
+    const long long base = blk0 + (long long)head * len;
+    const uint32_t q_addr = smem_u32(smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES);
+    const uint32_t do_addr = q_addr + Cfg::CHUNK_BYTES;
+    mbar_wait(&c_full[s], (ii / ATT_STAGES) & 1);
+    float st[32], dpt[32];
+    wgmma_fence();
+    mma_qk_64<BWD_D>(st, k_addr, Cfg::TILE_ATOM, q_addr, Cfg::CHUNK_ATOM);
+    if (DK) mma_qk_64<BWD_D>(dpt, v_addr, Cfg::TILE_ATOM, do_addr, Cfg::CHUNK_ATOM);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(st);
+    if (DK) reg_fence(dpt);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int q = qc0 + 8 * i + fp.c0;
+      const float l0 = q < len ? lse[base + q] * LOG2E : INFINITY, l1 = q + 1 < len ? lse[base + q + 1] * LOG2E : INFINITY;
+      float d0 = 0.f, d1 = 0.f;
+      if (DK) {
+        d0 = q < len ? delta[base + q] : 0.f;
+        d1 = q + 1 < len ? delta[base + q + 1] : 0.f;
+      }
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int qq = q + (e & 1);
+        // rows >= len belong to the next sequence (causality does not hide them: they come after the key)
+        const bool masked = kvr[e >> 1] > qq || qq >= len;
+        const float p = masked ? 0.f : fast_exp2(st[4 * i + e] * c - ((e & 1) ? l1 : l0));
+        st[4 * i + e] = masked ? 0.f : DK ? p * (dpt[4 * i + e] - ((e & 1) ? d1 : d0)) * scale : p;
+      }
+    }
+    uint32_t fa[4][4];
+    acc_to_afrag<4>(st, fa);
+    reg_fence(acc);
+    wgmma_fence();
+    mma_pv<BWD_D, 4>(acc, fa, DK ? q_addr : do_addr, Cfg::CHUNK_ATOM);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&c_empty[s]);
+  }
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_varlen_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                                const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dk,
+                                bf16* __restrict__ dv, long long ld_dkv, const int* __restrict__ cu, int n_heads,
+                                int kv_group, float scale) {
+  using Cfg = AttBwdCfg;
+  constexpr int D = BWD_D;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
+  uint64_t* kv_full = bars;
+  uint64_t* c_full = bars + 1;                  // [STAGES]
+  uint64_t* c_empty = bars + 1 + ATT_STAGES;    // [STAGES]
+
+  const int seq = blockIdx.z;
+  const int row0 = cu[seq], len = cu[seq + 1] - row0;
+  const int kv0 = blockIdx.x * 128;
+  if (kv0 >= len) return;
+  const int warp = threadIdx.x >> 5, wg = warp >> 2;
+  const int kv_head = blockIdx.y;
+  const int c_first = kv0 / BWD_C;                            // chunks holding a q >= kv0
+  const int n_c = (len + BWD_C - 1) / BWD_C - c_first;        // >= 1
+  const int n_it = n_c * kv_group;
+  const long long blk0 = (long long)n_heads * row0;
+
+  if (threadIdx.x == 0) {
+    mbar_init(kv_full, 1);
+    for (int i = 0; i < ATT_STAGES; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    if (threadIdx.x == 256) {
+      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
+      mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
+      for (int a = 0; a < 2; ++a) {
+        tma_load_2d(smem + a * Cfg::TILE_ATOM, &tmK, kv_full, kv_head * D + a * 64, row0 + kv0);
+        tma_load_2d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmV, kv_full, kv_head * D + a * 64, row0 + kv0);
+      }
+      for (int ii = 0; ii < 2 * n_it; ++ii) {
+        const int it = ii % n_it, s = ii % ATT_STAGES;
+        if (ii >= ATT_STAGES) mbar_wait(&c_empty[s], ((ii / ATT_STAGES) - 1) & 1);
+        const int qc0 = (c_first + it % n_c) * BWD_C;
+        const int head = kv_head * kv_group + it / n_c;
+        uint8_t* dst = smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES;
+        mbar_arrive_expect_tx(&c_full[s], 2 * Cfg::CHUNK_BYTES);
+        for (int a = 0; a < 2; ++a) {
+          tma_load_2d(dst + a * Cfg::CHUNK_ATOM, &tmQ, &c_full[s], head * D + a * 64, row0 + qc0);
+          tma_load_2d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmDO, &c_full[s], head * D + a * 64, row0 + qc0);
+        }
+      }
+    }
+  } else {
+    const FragPos fp = frag_pos();
+    const int kvr[2] = {kv0 + wg * 64 + fp.r0, kv0 + wg * 64 + fp.r0 + 8};
+    const float c = scale * LOG2E;
+    const uint32_t k_addr = smem_u32(smem) + wg * 64 * 128;
+    const uint32_t v_addr = smem_u32(smem + Cfg::OFF_T1) + wg * 64 * 128;
+    mbar_wait(kv_full, 0);
+    float acc[D / 2];
+#pragma unroll 1
+    for (int pass = 0; pass < 2; ++pass) {
+      if (pass == 0)
+        varlen_dkv_pass<false>(smem, c_full, c_empty, 0, n_it, n_c, c_first, kv_head, kv_group, blk0, len, kvr, k_addr,
+                               v_addr, c, scale, lse, delta, acc);
+      else
+        varlen_dkv_pass<true>(smem, c_full, c_empty, n_it, n_it, n_c, c_first, kv_head, kv_group, blk0, len, kvr,
+                              k_addr, v_addr, c, scale, lse, delta, acc);
+      bf16* dst = pass == 0 ? dv : dk;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int kv = kvr[h];
+        if (kv >= len) continue;
+        bf16* row = dst + ((long long)row0 + kv) * ld_dkv + kv_head * D + fp.c0;
+#pragma unroll
+        for (int i = 0; i < D / 8; ++i)
+          *reinterpret_cast<uint32_t*>(row + 8 * i) = pack_bf16(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_varlen_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                               const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                               const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dq,
+                               long long ld_dq, const int* __restrict__ cu, int n_heads, int kv_group, float scale) {
+  using Cfg = AttBwdCfg;
+  constexpr int D = BWD_D;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
+  uint64_t* q_full = bars;
+  uint64_t* c_full = bars + 1;
+  uint64_t* c_empty = bars + 1 + ATT_STAGES;
+
+  const int seq = blockIdx.z;
+  const int row0 = cu[seq], len = cu[seq + 1] - row0;
+  const int num_q_tiles = (len + 127) / 128;
+  if ((int)blockIdx.x >= num_q_tiles) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const int q_tile = num_q_tiles - 1 - blockIdx.x;            // heavy (late) tiles first
+  const int q0 = q_tile * 128;
+  const int head = blockIdx.y;
+  const int kv_head = head / kv_group;
+  const int n_c = min((len + BWD_C - 1) / BWD_C, (q0 + 128 + BWD_C - 1) / BWD_C);
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int i = 0; i < ATT_STAGES; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    if (threadIdx.x == 256) {
+      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
+      mbar_arrive_expect_tx(q_full, 2 * Cfg::TILE_BYTES);
+      for (int a = 0; a < 2; ++a) {
+        tma_load_2d(smem + a * Cfg::TILE_ATOM, &tmQ, q_full, head * D + a * 64, row0 + q0);
+        tma_load_2d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmDO, q_full, head * D + a * 64, row0 + q0);
+      }
+      for (int j = 0; j < n_c; ++j) {
+        const int s = j % ATT_STAGES;
+        if (j >= ATT_STAGES) mbar_wait(&c_empty[s], ((j / ATT_STAGES) - 1) & 1);
+        uint8_t* dst = smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES;
+        mbar_arrive_expect_tx(&c_full[s], 2 * Cfg::CHUNK_BYTES);
+        for (int a = 0; a < 2; ++a) {
+          tma_load_2d(dst + a * Cfg::CHUNK_ATOM, &tmK, &c_full[s], kv_head * D + a * 64, row0 + j * BWD_C);
+          tma_load_2d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmV, &c_full[s], kv_head * D + a * 64,
+                      row0 + j * BWD_C);
+        }
+      }
+    }
+  } else {
+    const FragPos fp = frag_pos();
+    const int qr[2] = {q0 + wg * 64 + fp.r0, q0 + wg * 64 + fp.r0 + 8};
+    const float c = scale * LOG2E;
+    const long long base = (long long)n_heads * row0 + (long long)head * len;
+    float lse2[2], dl[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      lse2[h] = qr[h] < len ? lse[base + qr[h]] * LOG2E : INFINITY;
+      dl[h] = qr[h] < len ? delta[base + qr[h]] : 0.f;
+    }
+    float dqacc[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) dqacc[i] = 0.f;
+    const uint32_t q_addr = smem_u32(smem) + wg * 64 * 128;
+    const uint32_t do_addr = smem_u32(smem + Cfg::OFF_T1) + wg * 64 * 128;
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < n_c; ++j) {
+      const int s = j % ATT_STAGES;
+      const uint32_t k_addr = smem_u32(smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES);
+      const uint32_t v_addr = k_addr + Cfg::CHUNK_BYTES;
+      mbar_wait(&c_full[s], (j / ATT_STAGES) & 1);
+      float sv[32], dp[32];
+      wgmma_fence();
+      mma_qk_64<D>(sv, q_addr, Cfg::TILE_ATOM, k_addr, Cfg::CHUNK_ATOM);
+      mma_qk_64<D>(dp, do_addr, Cfg::TILE_ATOM, v_addr, Cfg::CHUNK_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(sv);
+      reg_fence(dp);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int kv = j * BWD_C + 8 * i + fp.c0 + (e & 1);
+          const int h = e >> 1;
+          const bool masked = kv >= len || kv > qr[h];
+          const float p = masked ? 0.f : fast_exp2(sv[4 * i + e] * c - lse2[h]);
+          dp[4 * i + e] = p * (dp[4 * i + e] - dl[h]) * scale;
+        }
+      uint32_t da[4][4];
+      acc_to_afrag<4>(dp, da);
+      reg_fence(dqacc);
+      wgmma_fence();
+      mma_pv<D, 4>(dqacc, da, k_addr, Cfg::CHUNK_ATOM);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(dqacc);
+      if (lane == 0) mbar_arrive(&c_empty[s]);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int q = qr[h];
+      if (q >= len) continue;
+      bf16* row = dq + ((long long)row0 + q) * ld_dq + head * D + fp.c0;
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i)
+        *reinterpret_cast<uint32_t*>(row + 8 * i) = pack_bf16(dqacc[4 * i + 2 * h], dqacc[4 * i + 2 * h + 1]);
+    }
+  }
+}
+
+static int make_packed_tmap(CUtensorMap* tm, const void* ptr, long long ld, long long n_rows, int cols, int box_rows) {
+  uint64_t dims[2] = {(uint64_t)cols, (uint64_t)n_rows};
+  uint64_t str[1] = {(uint64_t)ld * 2};
+  uint32_t box[2] = {64, (uint32_t)box_rows};
+  return make_tmap_bf16(tm, ptr, 2, dims, str, box);
+}
+
+static int varlen_check(const char* who, long long ld_qkv, long long ld_out, void* out, int nseq, int max_len,
+                        long long n_rows, int n_heads, int n_kv_heads, int head_dim) {
+  B200_REQUIRE(head_dim == 128, "%s: head_dim must be 128 (got %d)", who, head_dim);
+  B200_REQUIRE(n_kv_heads > 0 && n_heads % n_kv_heads == 0, "%s: n_heads %d not a multiple of n_kv_heads %d", who,
+               n_heads, n_kv_heads);
+  B200_REQUIRE(nseq > 0 && max_len > 0 && n_rows > 0 && n_rows < 2147483647LL, "%s: bad shape", who);
+  B200_REQUIRE(ld_qkv % 8 == 0 && ld_out % 8 == 0 && ((uintptr_t)out & 15) == 0,
+               "%s: ld must be a multiple of 8 and out 16-byte aligned", who);
+  return 0;
+}
+
+}  // namespace b200
+
+// Packed causal self-attention: q/k/v/out [n_rows][ld] bf16 (q, k, v may be column blocks of one fused qkv buffer);
+// cu int32 [nseq + 1] (device) cuts the rows into sequences, max_len >= the longest; lse fp32 [n_heads * n_rows].
+extern "C" int rlaifv_attention_varlen_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out,
+                                           long long ld_out, float* lse, const int* cu, int nseq, int max_len,
+                                           long long n_rows, int n_heads, int n_kv_heads, int head_dim, float scale,
+                                           void* stream) {
+  int rc;
+  if ((rc = varlen_check("attention_varlen_fwd", ld_qkv, ld_out, out, nseq, max_len, n_rows, n_heads, n_kv_heads,
+                         head_dim)))
+    return rc;
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_packed_tmap(&tq, q, ld_qkv, n_rows, n_heads * head_dim, ATT_BQ))) return rc;
+  if ((rc = make_packed_tmap(&tk, k, ld_qkv, n_rows, n_kv_heads * head_dim, ATT_BKV))) return rc;
+  if ((rc = make_packed_tmap(&tv, v, ld_qkv, n_rows, n_kv_heads * head_dim, ATT_BKV))) return rc;
+  B200_CHECK_CUDA(configure_smem_once((const void*)attention_varlen_fwd_kernel, (int)AttFwdCfg<128>::SMEM_BYTES));
+  dim3 grid((max_len + ATT_BQ - 1) / ATT_BQ, n_heads, nseq);
+  attention_varlen_fwd_kernel<<<grid, ATT_THREADS, AttFwdCfg<128>::SMEM_BYTES, (cudaStream_t)stream>>>(
+      tq, tk, tv, (bf16*)out, ld_out, lse, cu, n_heads, n_heads / n_kv_heads, scale);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Its backward: delta, the dK/dV kernel, then the dQ kernel, which writes bf16 dQ [n_rows][ld_dq] (may be the q column
+// block of a fused dqkv buffer). dk/dv bf16 [n_rows][ld_dkv]; delta_ws fp32 [n_heads * n_rows]. Nothing needs zeroing.
+extern "C" int rlaifv_attention_varlen_bwd(const void* q, const void* k, const void* v, long long ld_qkv,
+                                           const void* out, long long ld_out, const void* d_out, long long ld_dout,
+                                           const float* lse, void* dq, long long ld_dq, void* dk, void* dv,
+                                           long long ld_dkv, float* delta_ws, const int* cu, int nseq, int max_len,
+                                           long long n_rows, int n_heads, int n_kv_heads, int head_dim, float scale,
+                                           void* stream) {
+  int rc;
+  if ((rc = varlen_check("attention_varlen_bwd", ld_qkv, ld_out, (void*)out, nseq, max_len, n_rows, n_heads,
+                         n_kv_heads, head_dim)))
+    return rc;
+  B200_REQUIRE(ld_dout % 8 == 0 && ((uintptr_t)d_out & 15) == 0, "attention_varlen_bwd: d_out must be 16-byte aligned");
+  B200_REQUIRE(dq != nullptr && ld_dq % 2 == 0 && ((uintptr_t)dq & 3) == 0 && ld_dkv % 2 == 0,
+               "attention_varlen_bwd: dq / dk / dv alignment");
+  const int g = n_heads / n_kv_heads;
+  CUtensorMap tq, tk, tv, tdo, tq2, tk2, tv2, tdo2;
+  if ((rc = make_packed_tmap(&tq, q, ld_qkv, n_rows, n_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_packed_tmap(&tdo, d_out, ld_dout, n_rows, n_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_packed_tmap(&tk, k, ld_qkv, n_rows, n_kv_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tv, v, ld_qkv, n_rows, n_kv_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tq2, q, ld_qkv, n_rows, n_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tdo2, d_out, ld_dout, n_rows, n_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tk2, k, ld_qkv, n_rows, n_kv_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_packed_tmap(&tv2, v, ld_qkv, n_rows, n_kv_heads * head_dim, BWD_C))) return rc;
+  B200_CHECK_CUDA(configure_smem_once((const void*)attention_varlen_bwd_dkv_kernel, (int)AttBwdCfg::SMEM_BYTES));
+  B200_CHECK_CUDA(configure_smem_once((const void*)attention_varlen_bwd_dq_kernel, (int)AttBwdCfg::SMEM_BYTES));
+  cudaStream_t st = (cudaStream_t)stream;
+  {
+    const long long total = n_rows * n_heads;
+    long long blocks = (total + 7) / 8;
+    if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
+    attention_varlen_delta_kernel<<<(int)blocks, 256, 0, st>>>((const bf16*)out, ld_out, (const bf16*)d_out, ld_dout,
+                                                               delta_ws, cu, nseq, n_rows, n_heads, head_dim);
+    B200_CHECK_CUDA(cudaGetLastError());
+  }
+  {
+    dim3 grid((max_len + 127) / 128, n_kv_heads, nseq);
+    attention_varlen_bwd_dkv_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
+        tq, tk, tv, tdo, lse, delta_ws, (bf16*)dk, (bf16*)dv, ld_dkv, cu, n_heads, g, scale);
+    B200_CHECK_CUDA(cudaGetLastError());
+  }
+  {
+    dim3 grid((max_len + 127) / 128, n_heads, nseq);
+    attention_varlen_bwd_dq_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
+        tq2, tk2, tv2, tdo2, lse, delta_ws, (bf16*)dq, ld_dq, cu, n_heads, g, scale);
+    B200_CHECK_CUDA(cudaGetLastError());
+  }
+  return 0;
+}

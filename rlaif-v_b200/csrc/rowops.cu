@@ -427,6 +427,69 @@ __global__ void rope_bwd_kernel(bf16* __restrict__ dqkv, const float* __restrict
   }
 }
 
+// RoPE of packed rows: rope_fwd_kernel / rope_bwd_kernel (split form: dQ already in the q block) with the position of
+// row m read from pos[m] instead of m % T.
+__global__ void rope_pos_fwd_kernel(bf16* __restrict__ qkv, const bf16* __restrict__ cosb, const bf16* __restrict__ sinb,
+                                    const int* __restrict__ pos_of, long long M, int nrot, int D, long long ld) {
+  const int half = D >> 1;
+  const int per_head = half >> 3;
+  const long long total = M * nrot * per_head;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int c8 = (int)(idx % per_head);
+    long long r = idx / per_head;
+    const int head = (int)(r % nrot);
+    const long long row = r / nrot;
+    const int pos = pos_of[row];
+    bf16* p = qkv + row * ld + (long long)head * D + c8 * 8;
+    float x1[8], x2[8], c1[8], s1[8], c2[8], s2[8];
+    load8(p, x1);
+    load8(p + half, x2);
+    load8(cosb + (long long)pos * D + c8 * 8, c1);
+    load8(sinb + (long long)pos * D + c8 * 8, s1);
+    load8(cosb + (long long)pos * D + half + c8 * 8, c2);
+    load8(sinb + (long long)pos * D + half + c8 * 8, s2);
+    float o1[8], o2[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      o1[j] = bf16_round(x1[j] * c1[j]) + bf16_round(-x2[j] * s1[j]);
+      o2[j] = bf16_round(x2[j] * c2[j]) + bf16_round(x1[j] * s2[j]);
+    }
+    store8(p, o1);
+    store8(p + half, o2);
+  }
+}
+__global__ void rope_pos_bwd_kernel(bf16* __restrict__ dqkv, const bf16* __restrict__ cosb, const bf16* __restrict__ sinb,
+                                    const int* __restrict__ pos_of, long long M, int nrot, int D, long long ld) {
+  const int half = D >> 1;
+  const int per_head = half >> 3;
+  const long long total = M * nrot * per_head;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int c8 = (int)(idx % per_head);
+    long long r = idx / per_head;
+    const int head = (int)(r % nrot);
+    const long long row = r / nrot;
+    const int pos = pos_of[row];
+    bf16* p = dqkv + row * ld + (long long)head * D + c8 * 8;
+    float y1[8], y2[8], c1[8], s1[8], c2[8], s2[8];
+    load8(p, y1);
+    load8(p + half, y2);
+    load8(cosb + (long long)pos * D + c8 * 8, c1);
+    load8(sinb + (long long)pos * D + c8 * 8, s1);
+    load8(cosb + (long long)pos * D + half + c8 * 8, c2);
+    load8(sinb + (long long)pos * D + half + c8 * 8, s2);
+    float o1[8], o2[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      o1[j] = y1[j] * c1[j] + y2[j] * s2[j];
+      o2[j] = y2[j] * c2[j] - y1[j] * s1[j];
+    }
+    store8(p, o1);
+    store8(p + half, o2);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // SwiGLU (HF llama/modeling_llama.py:182-184): act = bf16(bf16(silu(g)) * u), gu = [g | u] per row
 // ------------------------------------------------------------------------------------------------
@@ -1176,6 +1239,31 @@ __global__ void dropout_bwd_add_kernel(bf16* __restrict__ dx, const bf16* __rest
     store8(dx + idx * 8, a);
   }
 }
+// Dropout of packed rows [n_rows][w8 * 8]: row r draws the keep bits of element (rows[r] * w8 * 8 + c), i.e. those of
+// the padded row rows[r] in dropout_fwd_kernel / dropout_bwd_add_kernel. bwd: g == nullptr => forward (out = mask(x)).
+__global__ void dropout_rows_kernel(const bf16* x, const bf16* __restrict__ g, bf16* out,
+                                    const int* __restrict__ rows, long long n_rows, int w8, uint32_t thresh,
+                                    float inv_keep, unsigned long long seed) {
+  const long long n8 = n_rows * w8;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < n8;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const long long r = idx / w8;
+    const long long chunk = (long long)rows[r] * w8 + (idx - r * w8);
+    float a[8], b[8];
+    bool keep[8];
+    load8(x + idx * 8, a);
+    keep_bits8(seed, chunk, thresh, keep);
+    if (g) {
+      load8(g + idx * 8, b);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) a[j] += keep[j] ? b[j] * inv_keep : 0.f;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) a[j] = keep[j] ? a[j] * inv_keep : 0.f;
+    }
+    store8(out + idx * 8, a);
+  }
+}
 
 static inline int grid_for(long long work_items, int threads, int max_blocks_per_sm = 8) {
   long long blocks = (work_items + threads - 1) / threads;
@@ -1289,6 +1377,28 @@ extern "C" int rlaifv_rope_bwd_gqa(void* dqkv, const float* dq_f32, const void* 
                                    long long M, int T, int n_heads, int n_kv_heads, int head_dim, long long ld,
                                    void* stream) {
   return rope_bwd_impl(dqkv, dq_f32, cos_tab, sin_tab, M, T, n_heads, n_kv_heads, head_dim, ld, stream);
+}
+
+// RoPE of packed rows: the position of row m is pos[m] (int32 [M], device); backward in the split form only.
+extern "C" int rlaifv_rope_pos_fwd(void* qkv, const void* cos_tab, const void* sin_tab, const int* pos, long long M,
+                                   int n_heads, int n_kv_heads, int head_dim, long long ld, void* stream) {
+  B200_REQUIRE(head_dim % 16 == 0 && M > 0, "rope_pos_fwd: head_dim %% 16 != 0 or M <= 0");
+  const int nrot = n_heads + n_kv_heads;
+  const long long total = M * nrot * (head_dim / 16);
+  rope_pos_fwd_kernel<<<grid_for(total, 256), 256, 0, ST>>>((bf16*)qkv, (const bf16*)cos_tab, (const bf16*)sin_tab, pos,
+                                                            M, nrot, head_dim, ld);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+extern "C" int rlaifv_rope_pos_bwd(void* dqkv, const void* cos_tab, const void* sin_tab, const int* pos, long long M,
+                                   int n_heads, int n_kv_heads, int head_dim, long long ld, void* stream) {
+  B200_REQUIRE(head_dim % 16 == 0 && M > 0, "rope_pos_bwd: head_dim %% 16 != 0 or M <= 0");
+  const int nrot = n_heads + n_kv_heads;
+  const long long total = M * nrot * (head_dim / 16);
+  rope_pos_bwd_kernel<<<grid_for(total, 256), 256, 0, ST>>>((bf16*)dqkv, (const bf16*)cos_tab, (const bf16*)sin_tab, pos,
+                                                            M, nrot, head_dim, ld);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
 }
 
 extern "C" int rlaifv_swiglu_fwd(const void* gu, void* act, long long M, int F, void* stream) {
@@ -1663,6 +1773,22 @@ extern "C" int rlaifv_dropout_bwd_add(void* dx, const void* g, long long n, floa
   B200_REQUIRE(n % 8 == 0 && p >= 0.f && p < 1.f, "dropout_bwd_add: n %% 8 != 0 or p outside [0,1)");
   dropout_bwd_add_kernel<<<grid_for(n / 8, 256), 256, 0, ST>>>((bf16*)dx, (const bf16*)g, n / 8, dropout_threshold(p),
                                                                1.f / (1.f - p), seed);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+extern "C" int rlaifv_dropout_rows_fwd(const void* x, void* out, const int* rows, long long n_rows, int width, float p,
+                                       unsigned long long seed, void* stream) {
+  B200_REQUIRE(width % 8 == 0 && n_rows > 0 && p >= 0.f && p < 1.f, "dropout_rows_fwd: width %% 8 != 0 or bad p");
+  dropout_rows_kernel<<<grid_for(n_rows * (width / 8), 256), 256, 0, ST>>>(
+      (const bf16*)x, nullptr, (bf16*)out, rows, n_rows, width / 8, dropout_threshold(p), 1.f / (1.f - p), seed);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+extern "C" int rlaifv_dropout_rows_bwd_add(void* dx, const void* g, const int* rows, long long n_rows, int width,
+                                           float p, unsigned long long seed, void* stream) {
+  B200_REQUIRE(width % 8 == 0 && n_rows > 0 && p >= 0.f && p < 1.f, "dropout_rows_bwd_add: width %% 8 != 0 or bad p");
+  dropout_rows_kernel<<<grid_for(n_rows * (width / 8), 256), 256, 0, ST>>>(
+      (const bf16*)dx, (const bf16*)g, (bf16*)dx, rows, n_rows, width / 8, dropout_threshold(p), 1.f / (1.f - p), seed);
   B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

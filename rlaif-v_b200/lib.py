@@ -98,6 +98,15 @@ _SIGNATURES = {
     "rlaifv_logp_weighted_reduce": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "rlaifv_splice_map_inplace": [c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_void_p, c_void_p,
                                   c_void_p],
+    "rlaifv_attention_varlen_fwd": [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p, c_int,
+                                    c_int, c_ll, c_int, c_int, c_int, c_float, c_void_p],
+    "rlaifv_attention_varlen_bwd": [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p,
+                                    c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_ll,
+                                    c_int, c_int, c_int, c_float, c_void_p],
+    "rlaifv_rope_pos_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_void_p],
+    "rlaifv_rope_pos_bwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_void_p],
+    "rlaifv_dropout_rows_fwd": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, ctypes.c_ulonglong, c_void_p],
+    "rlaifv_dropout_rows_bwd_add": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, ctypes.c_ulonglong, c_void_p],
 }
 _INT_RETURNING_PLAIN = {"rlaifv_rmsnorm_bwd_partials": []}
 

@@ -257,6 +257,49 @@ class LoraStore(FlatStore):
         return out
 
 
+@dataclass
+class RowPacking:
+    """Packed rows of a training forward (DESIGN.md §3). Sequence s keeps its first len_s rows, len_s = 1 + the last
+    position whose spliced label is supervised (1 if there is none): attention is causal, so no supervised log-prob
+    depends on a later row, and the compact head gives those rows exactly zero gradient. Sequence s occupies packed
+    rows [cu[s], cu[s] + len_s); packed row cu[s] + t is position t."""
+    nseq: int
+    T: int                   # padded length
+    M: int                   # packed rows: sum of len_s
+    max_len: int             # longest len_s
+    cu: torch.Tensor         # int32 [nseq + 1]
+    pos: torch.Tensor        # int32 [M]: position t of each packed row (its RoPE position)
+    rows: torch.Tensor       # int32 [M]: the padded row s*T + t of each packed row
+
+    def packed_rows(self, row_pos):
+        """Padded rows s*T + t (-1 = unused slot, kept) -> packed rows cu[s] + t."""
+        rp = row_pos.long().clamp(min=0)
+        s = torch.div(rp, self.T, rounding_mode="floor")
+        return torch.where(row_pos >= 0, self.cu.long()[s] + rp - s * self.T, -1).to(torch.int32)
+
+
+def packed_lengths(labels):
+    """len_s of spliced labels [nseq, T] (int64): 1 + the last supervised position, 1 if none."""
+    t = torch.arange(labels.shape[1], device=labels.device)
+    return (torch.where(labels != IGNORE_INDEX, t, -1).amax(dim=1) + 1).clamp(min=1)
+
+
+def pack_rows(labels):
+    """RowPacking of spliced labels [nseq, T], or None when every len_s is T. Reads the lengths to the host once."""
+    nseq, T = labels.shape
+    lens = packed_lengths(labels)
+    lens_h = lens.cpu()
+    M = int(lens_h.sum())
+    if M == nseq * T:
+        return None
+    dev = labels.device
+    cu = torch.zeros(nseq + 1, dtype=torch.int64, device=dev)
+    cu[1:] = torch.cumsum(lens, 0)
+    seq = torch.repeat_interleave(torch.arange(nseq, device=dev), lens, output_size=M)
+    pos = torch.arange(M, device=dev) - cu[seq]
+    return RowPacking(nseq, T, M, int(lens_h.max()), cu.int(), pos.int(), (seq * T + pos).int())
+
+
 class ClipWeights:
     """Frozen CLIP-ViT weights in kernel-friendly form (fused qkv, padded patch-embedding matrix)."""
 
@@ -346,6 +389,10 @@ class LlavaDPOPolicy:
         self.compact_head = True
         # attention backward as two kernels (dK/dV, dQ) without fp32 atomics; False = the fused round-1 kernel
         self.split_attention_bwd = True
+        # ragged training batches run the decoder on packed rows (RowPacking) when that drops any row; False = always
+        # the padded layout (the reference the packed path is tested against). A policy on the CPU only serves host-side
+        # dry runs of the padded launch sequence, so it packs only when asked.
+        self.pack_rows = self.device.type == "cuda"
         # SwiGLU backward inside the epilogue of the down-projection dgrad (no d(act) round trip, one launch less per
         # layer); False = separate swiglu_bwd pass
         self.fuse_swiglu_bwd = True
@@ -420,7 +467,8 @@ class LlavaDPOPolicy:
         if L.dropout > 0.0 and self.training and ls is not None:
             # the sub-linears of a fused group share one mask (peft draws one per adapter; same marginal law)
             seed = self._lora_seed(i, group)
-            xa = ops.dropout_fwd(x, L.dropout, seed, out=self.buf("lora_xd_%d" % x.shape[1], tuple(x.shape)))
+            xa = ops.dropout_fwd(x, L.dropout, seed, out=self.buf("lora_xd_%d" % x.shape[1], tuple(x.shape)),
+                                 rows=ls.get("rows"))
             ls["seed_" + group] = seed
         ops.gemm(xa, A, t, alpha=L.scaling)
         n_sub = out.shape[1] // len(b_names) if len(b_names) > 1 else 0
@@ -453,12 +501,13 @@ class LlavaDPOPolicy:
         seed = ls.get("seed_" + group)
         if seed is not None:
             # dropout on the adapter input: dA sees the dropped input, and the adapter's dx passes through the mask
-            xd = ops.dropout_fwd(x, L.dropout, seed, out=self.buf("lora_xd_%d" % x.shape[1], tuple(x.shape)))
+            xd = ops.dropout_fwd(x, L.dropout, seed, out=self.buf("lora_xd_%d" % x.shape[1], tuple(x.shape)),
+                                 rows=ls.get("rows"))
             ops.gemm(dt, xd, L.g[f"l{i}.{a_name}"], a_mn=True, b_mn=True, accumulate=acc)             # dA = dt^T drop(x)
             dx_plain = dx_out if glu is None else self.buf("dact", tuple(x.shape))
             ops.gemm(dy, W, dx_plain, b_mn=True)
             pa = ops.gemm(dt, A, self.buf("lora_xd_%d" % x.shape[1], tuple(x.shape)), b_mn=True)                       # dt @ A
-            ops.dropout_bwd_add(dx_plain, pa, L.dropout, seed)
+            ops.dropout_bwd_add(dx_plain, pa, L.dropout, seed, rows=ls.get("rows"))
             return dx_plain if glu is None else ops.swiglu_bwd(glu, dx_plain, dx_out)
         ops.gemm(dt, x, L.g[f"l{i}.{a_name}"], a_mn=True, b_mn=True, accumulate=acc)                  # dA = dt^T x
         # dx = dy @ W + dt @ A in one pass (second source = stacked lora_A, MN-major like W)
@@ -551,22 +600,24 @@ class LlavaDPOPolicy:
         return embeds, new_labels, src, T
 
     # ------------------------------------------------------------------ decoder layers
-    def _run_layers(self, x, nseq, T, st):
+    def _run_layers(self, x, nseq, T, st, pk=None):
         """32 x [RMSNorm -> fused qkv GEMM -> RoPE -> causal attention -> o GEMM(+res) -> RMSNorm ->
-        fused gate|up GEMM -> SwiGLU -> down GEMM(+res)]; st (dict or None) receives the per-layer stash."""
+        fused gate|up GEMM -> SwiGLU -> down GEMM(+res)]; st (dict or None) receives the per-layer stash.
+        pk (RowPacking): x holds the packed rows, attention and RoPE run variable-length."""
         d, P, dev = self.dims, self.store.p, self.device
         H, F, KV = d.hidden_size, d.intermediate_size, d.kv_size
         nh, hd, nkv = d.num_heads, d.head_dim, d.kv_heads
         QKV = H + 2 * KV
-        M = nseq * T
+        M = nseq * T if pk is None else pk.M
         cos, sin = self.rope_tables(T)
         scale = hd ** -0.5
         keep_stash = st is not None
+        lse_shape = (nseq, nh, T) if pk is None else (nh * M,)
         for i in range(d.num_layers):
             self._need(self.layer_bucket_name(i))
             ls = None
             if keep_stash:
-                ls = {"x": x}
+                ls = {"x": x} if pk is None else {"x": x, "rows": pk.rows}
                 qkv = torch.empty((M, QKV), dtype=_BF, device=dev)
                 att = torch.empty((M, H), dtype=_BF, device=dev)
                 x2 = torch.empty((M, H), dtype=_BF, device=dev)
@@ -574,21 +625,26 @@ class LlavaDPOPolicy:
                 x3 = torch.empty((M, H), dtype=_BF, device=dev)
                 rstd1 = torch.empty(M, dtype=_F32, device=dev)
                 rstd2 = torch.empty(M, dtype=_F32, device=dev)
-                lse = torch.empty((nseq, nh, T), dtype=_F32, device=dev)
+                lse = torch.empty(lse_shape, dtype=_F32, device=dev)
             else:
                 qkv, att = self.buf("qkv", (M, QKV)), self.buf("att", (M, H))
                 x2, gu = self.buf("x2", (M, H)), self.buf("gu", (M, 2 * F))
                 x3 = self.buf("x3_%d" % (i & 1), (M, H))
                 rstd1 = rstd2 = None
-                lse = self.buf("lse", (nseq, nh, T), _F32)
+                lse = self.buf("lse", lse_shape, _F32)
             extra = keep_stash and self.stash_extra
             n1 = ops.rmsnorm_fwd(x, P[f"l{i}.ln1"], d.rms_eps,
                                  out=torch.empty((M, H), dtype=_BF, device=dev) if extra else self.buf("n", (M, H)),
                                  rstd=rstd1)
             self._lin_fwd(i, "qkv", n1, qkv, ls=ls if keep_stash else None)
-            ops.rope_fwd(qkv, cos, sin, T, nh, hd, n_kv_heads=nkv)
-            ops.attention_fwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], nseq, T, nh, hd, True, scale, out=att,
-                              lse=lse, n_kv_heads=nkv)
+            if pk is None:
+                ops.rope_fwd(qkv, cos, sin, T, nh, hd, n_kv_heads=nkv)
+                ops.attention_fwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], nseq, T, nh, hd, True, scale, out=att,
+                                  lse=lse, n_kv_heads=nkv)
+            else:
+                ops.rope_pos_fwd(qkv, cos, sin, pk.pos, nh, hd, n_kv_heads=nkv)
+                ops.attention_varlen_fwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], pk, nh, hd, scale, att, lse,
+                                         n_kv_heads=nkv)
             self._lin_fwd(i, "o", att, x2, residual=x, ls=ls if keep_stash else None)
             n2 = ops.rmsnorm_fwd(x2, P[f"l{i}.ln2"], d.rms_eps,
                                  out=torch.empty((M, H), dtype=_BF, device=dev) if extra else self.buf("n", (M, H)),
@@ -641,20 +697,26 @@ class LlavaDPOPolicy:
         self._need("embed")
         x, new_labels, src, T = self.splice(input_ids, labels, proj, b, img_index,
                                             T_hint=(T_hint, n_slots) if T_hint is not None else None)
+        compact = keep_stash and self.compact_head
+        # training on a ragged batch: the decoder runs only each sequence's rows up to its last supervised position
+        pk = pack_rows(new_labels) if compact and self.pack_rows else None
+        if pk is not None:
+            x = ops.rows_gather(pk.rows, x, out=self.buf("xp", (pk.M, H)))
         if keep_stash:
             st.update(src=src, input_ids=input_ids, labels=new_labels, T=T, nseq=nseq, b=b,
-                      n_feat_rows=proj.shape[0])
-        x = self._run_layers(x, nseq, T, st)
+                      n_feat_rows=proj.shape[0], pack=pk)
+        x = self._run_layers(x, nseq, T, st, pk)
         self._need("head")
-        compact = keep_stash and self.compact_head
         row_pos = None
         if compact:
             # training: only the positions whose next token is supervised reach the final norm / lm_head / log-softmax
             # (get_batch_logps masks the rest out of the sum, muffin_inference_logp.py:93-104). A row of the collator
             # holds at most L labels, so L slots per sequence always suffice — no host sync for the count.
+            # row_pos (padded positions) locates labels / per_tok; x_rows locates the rows of x.
             row_pos = ops.supervised_rows(new_labels, input_ids.shape[1])
-            x = ops.rows_gather(row_pos, x, out=self.buf("xc", (row_pos.numel(), H)))
-            st["row_pos"] = row_pos
+            x_rows = row_pos if pk is None else pk.packed_rows(row_pos)
+            x = ops.rows_gather(x_rows, x, out=self.buf("xc", (row_pos.numel(), H)))
+            st.update(row_pos=row_pos, x_rows=x_rows)
         R, sfx = x.shape[0], "_c" if compact else ""      # rows that reach the head (M, or the compact row count)
         rstd_f = torch.empty(R, dtype=_F32, device=dev) if keep_stash else None
         hn = ops.rmsnorm_fwd(x, P["norm"], d.rms_eps, out=self.buf("hn" + sfx, (R, H)), rstd=rstd_f)
@@ -674,8 +736,8 @@ class LlavaDPOPolicy:
         assert st is not None, "forward_logps(keep_stash=True) must precede backward_logps"
         d, P, G = self.dims, self.store.p, self.store.g
         dev = self.device
-        nseq, T, b = st["nseq"], st["T"], st["b"]
-        M = nseq * T
+        nseq, T, b, pk = st["nseq"], st["T"], st["b"], st["pack"]
+        M = nseq * T if pk is None else pk.M
         H, F, V, KV = d.hidden_size, d.intermediate_size, d.vocab_size, d.kv_size
         nh, hd, nkv = d.num_heads, d.head_dim, d.kv_heads
         scale = hd ** -0.5
@@ -700,7 +762,7 @@ class LlavaDPOPolicy:
         if row_pos is not None:                   # back to the [M, H] residual stream (zeros at unsupervised positions)
             full = self.buf("dx_a", (M, H))
             full.zero_()
-            dx = ops.rows_scatter(row_pos, dx, full)
+            dx = ops.rows_scatter(st["x_rows"], dx, full)
         if self.on_head_grads_ready is not None:
             self.on_head_grads_ready()
         for i in reversed(range(d.num_layers)):
@@ -722,7 +784,12 @@ class LlavaDPOPolicy:
             datt = self._lin_bwd(i, "o", dx2, ls["att"], self.buf("datt", (M, H)), ls, acc)
             qkv = ls["qkv"]
             dqkv = self.buf("dqkv", (M, H + 2 * KV))
-            if self.split_attention_bwd:
+            if pk is not None:
+                ops.attention_varlen_bwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], ls["att"], datt, ls["lse"], pk,
+                                         nh, hd, scale, dqkv[:, :H], dqkv[:, H:H + KV], dqkv[:, H + KV:],
+                                         self.buf("delta", (nh * M,), _F32), n_kv_heads=nkv)
+                ops.rope_pos_bwd(dqkv, cos, sin, pk.pos, nh, hd, n_kv_heads=nkv)
+            elif self.split_attention_bwd:
                 # dK/dV kernel + dQ kernel: dQ lands in the q block of dqkv as bf16, rotated back in place
                 ops.attention_bwd_split(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], ls["att"], datt, ls["lse"], nseq,
                                         T, T, nh, hd, True, scale, dqkv[:, :H], dqkv[:, H:H + KV], dqkv[:, H + KV:],
@@ -753,7 +820,15 @@ class LlavaDPOPolicy:
         n_feat_rows = st["n_feat_rows"]
         dfeat32 = self.buf("dfeat32", (n_feat_rows, H), _F32)
         dfeat32.zero_()
-        ops.splice_scatter(st["src"], st["input_ids"], dx, None if frozen else self.embed_grad_f32, dfeat32)
+        src, ids = st["src"], st["input_ids"]
+        if pk is not None:
+            # scatter straight from the packed rows: one "sequence" of M rows over the flattened ids, a token's source
+            # index offset by its sequence's start in them
+            L = ids.shape[1]
+            src = src.view(-1)[pk.rows.long()]
+            src = torch.where(src >= 0, src + torch.div(pk.rows, T, rounding_mode="floor") * L, src).view(1, -1)
+            ids = ids.view(1, -1)
+        ops.splice_scatter(src, ids, dx, None if frozen else self.embed_grad_f32, dfeat32)
         dproj = ops.f32_to_bf16(dfeat32, self.buf("dproj", (n_feat_rows, H)))
         self._frontend_bwd(dproj, st, acc)
         self._stash = None

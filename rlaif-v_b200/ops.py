@@ -112,6 +112,31 @@ def attention_bwd_split(q, k, v, out, d_out, lse, nseq, Sq, Skv, n_heads, head_d
     return dq, dk, dv
 
 
+def attention_varlen_fwd(q, k, v, pk, n_heads, head_dim, scale, out, lse, n_kv_heads=None):
+    """Causal attention of packed rows (pk: model.RowPacking): q/k/v [pk.M, ld] views sharing one row stride,
+    out [pk.M, n_heads*head_dim], lse fp32 [n_heads*pk.M] (sequence s's [n_heads][len_s] block at n_heads*cu[s])."""
+    _chk(q), _chk(k), _chk(v), _chk(out), _chk(lse, _f32)
+    assert q.stride(0) == k.stride(0) == v.stride(0) and q.stride(1) == 1 and lse.numel() == n_heads * pk.M
+    _l.call("rlaifv_attention_varlen_fwd", _l.ptr(q), _l.ptr(k), _l.ptr(v), q.stride(0), _l.ptr(out), out.stride(0),
+            _l.ptr(lse), _l.ptr(pk.cu), pk.nseq, pk.max_len, pk.M, n_heads,
+            n_heads if n_kv_heads is None else n_kv_heads, head_dim, float(scale), _l.stream_ptr())
+    return out, lse
+
+
+def attention_varlen_bwd(q, k, v, out, d_out, lse, pk, n_heads, head_dim, scale, dq, dk, dv, delta_ws,
+                         n_kv_heads=None):
+    """Backward of attention_varlen_fwd (split form): dq bf16 [pk.M, n_heads*head_dim] (may be the q column block of a
+    fused dqkv buffer), dk/dv bf16 views sharing a row stride, delta_ws fp32 [n_heads*pk.M]. Nothing needs zeroing."""
+    _chk(q), _chk(k), _chk(v), _chk(out), _chk(d_out), _chk(dq), _chk(dk), _chk(dv), _chk(lse, _f32)
+    _chk(delta_ws, _f32)
+    assert q.stride(0) == k.stride(0) == v.stride(0) and dk.stride(0) == dv.stride(0) and dq.stride(1) == 1
+    _l.call("rlaifv_attention_varlen_bwd", _l.ptr(q), _l.ptr(k), _l.ptr(v), q.stride(0), _l.ptr(out), out.stride(0),
+            _l.ptr(d_out), d_out.stride(0), _l.ptr(lse), _l.ptr(dq), dq.stride(0), _l.ptr(dk), _l.ptr(dv),
+            dk.stride(0), _l.ptr(delta_ws), _l.ptr(pk.cu), pk.nseq, pk.max_len, pk.M, n_heads,
+            n_heads if n_kv_heads is None else n_kv_heads, head_dim, float(scale), _l.stream_ptr())
+    return dq, dk, dv
+
+
 def cross_attention_fwd(q, k, v, nseq, Sq, Skv, n_heads, head_dim, scale, q_shared=True, out=None, lse=None):
     """Non-causal cross-attention: q [(1 if q_shared else nseq)*Sq, ld_q], k/v [nseq*Skv, ld_kv] (column blocks of
     one buffer allowed) -> out [nseq*Sq, n_heads*head_dim], lse [nseq, n_heads, Sq]."""
@@ -225,6 +250,24 @@ def rope_bwd(dqkv, dq_f32, cos, sin, T, n_heads, head_dim, n_kv_heads=None):
         _chk(dq_f32, _f32)
     _l.call("rlaifv_rope_bwd_gqa", _l.ptr(dqkv), _l.ptr(dq_f32), _l.ptr(cos), _l.ptr(sin), dqkv.shape[0], T,
             n_heads, n_heads if n_kv_heads is None else n_kv_heads, head_dim, dqkv.stride(0), _l.stream_ptr())
+    return dqkv
+
+
+def rope_pos_fwd(qkv, cos, sin, pos, n_heads, head_dim, n_kv_heads=None):
+    """RoPE in place on fused qkv rows whose positions are pos (int32 [M]) — the packed rows' form of rope_fwd."""
+    _chk(qkv), _chk(cos), _chk(sin), _chk(pos, torch.int32)
+    assert pos.numel() == qkv.shape[0]
+    _l.call("rlaifv_rope_pos_fwd", _l.ptr(qkv), _l.ptr(cos), _l.ptr(sin), _l.ptr(pos), qkv.shape[0], n_heads,
+            n_heads if n_kv_heads is None else n_kv_heads, head_dim, qkv.stride(0), _l.stream_ptr())
+    return qkv
+
+
+def rope_pos_bwd(dqkv, cos, sin, pos, n_heads, head_dim, n_kv_heads=None):
+    """Inverse rotation in place of the q (bf16 dQ of the split backward) and k blocks of dqkv at positions pos."""
+    _chk(dqkv), _chk(cos), _chk(sin), _chk(pos, torch.int32)
+    assert pos.numel() == dqkv.shape[0]
+    _l.call("rlaifv_rope_pos_bwd", _l.ptr(dqkv), _l.ptr(cos), _l.ptr(sin), _l.ptr(pos), dqkv.shape[0], n_heads,
+            n_heads if n_kv_heads is None else n_kv_heads, head_dim, dqkv.stride(0), _l.stream_ptr())
     return dqkv
 
 
@@ -533,18 +576,31 @@ def gemm_swiglu_bwd(dy, w, gu, dgu, *, b_mn=True, a2=None, b2=None):
     return dgu
 
 
-def dropout_fwd(x, p, seed, out=None):
+def dropout_fwd(x, p, seed, out=None, rows=None):
+    """rows (int32 [M], packed rows): row r of x [M, width] draws the mask of row rows[r] of the padded layout."""
     _chk(x)
     assert x.is_contiguous()
     if out is None:
         out = torch.empty_like(x)
+    if rows is not None:
+        _chk(rows, torch.int32)
+        assert rows.numel() == x.shape[0]
+        _l.call("rlaifv_dropout_rows_fwd", _l.ptr(x), _l.ptr(out), _l.ptr(rows), x.shape[0], x.shape[1], float(p),
+                int(seed), _l.stream_ptr())
+        return out
     _l.call("rlaifv_dropout_fwd", _l.ptr(x), _l.ptr(out), x.numel(), float(p), int(seed), _l.stream_ptr())
     return out
 
 
-def dropout_bwd_add(dx, g, p, seed):
-    """dx += mask(seed) * g / (1 - p), the mask of dropout_fwd with the same seed."""
+def dropout_bwd_add(dx, g, p, seed, rows=None):
+    """dx += mask(seed) * g / (1 - p), the mask of dropout_fwd with the same seed (and rows)."""
     _chk(dx), _chk(g)
     assert dx.is_contiguous() and g.is_contiguous() and dx.numel() == g.numel()
+    if rows is not None:
+        _chk(rows, torch.int32)
+        assert rows.numel() == dx.shape[0]
+        _l.call("rlaifv_dropout_rows_bwd_add", _l.ptr(dx), _l.ptr(g), _l.ptr(rows), dx.shape[0], dx.shape[1], float(p),
+                int(seed), _l.stream_ptr())
+        return dx
     _l.call("rlaifv_dropout_bwd_add", _l.ptr(dx), _l.ptr(g), dx.numel(), float(p), int(seed), _l.stream_ptr())
     return dx
