@@ -200,6 +200,39 @@ reduce_partials_kernel(const float* __restrict__ part, int P, int H, bf16* __res
 // LayerNorm forward (CLIP; HF clip/modeling_clip.py pre_layrnorm / layer_norm1/2): fp32 stats,
 // y = bf16((x-mean)*rstd*w + b)
 // ------------------------------------------------------------------------------------------------
+// Mean and rstd of one register-cached row (H <= NORM_THREADS * 8 * NORM_MAXCH). One pass gives the mean and
+// E[x^2] - mean^2. That difference cancels in fp32 when |mean| >> std (a row of 100.0 with 1 in 512 elements one bf16 ulp
+// higher gave a variance of 0 and an rstd of eps^-1/2), so when mean^2 exceeds it the variance is taken again as the
+// mean of (x - mean)^2 over the cached row. A one-pass variance that is at least mean^2 has lost at most a factor ~2 of
+// the sum's rounding (E[x^2] <= 2 var), and rows of that kind get the same bits as the one-pass kernel always gave.
+// The test is on block-reduced values, so the whole block takes the same branch.
+__device__ __forceinline__ float2 layernorm_stats(const float (&xv)[NORM_MAXCH][8], int nch, int H, float eps) {
+  float s = 0.f, ss = 0.f;
+#pragma unroll
+  for (int ci = 0; ci < NORM_MAXCH; ++ci)
+    if (threadIdx.x + ci * NORM_THREADS < nch) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { s += xv[ci][j]; ss += xv[ci][j] * xv[ci][j]; }
+    }
+  const float2 tot = block_sum2(s, ss);
+  const float mean = tot.x / (float)H;
+  float var = fmaxf(tot.y / (float)H - mean * mean, 0.f);
+  if (__fmul_rn(mean, mean) > var) {
+    float dd = 0.f;
+#pragma unroll
+    for (int ci = 0; ci < NORM_MAXCH; ++ci)
+      if (threadIdx.x + ci * NORM_THREADS < nch) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float d = xv[ci][j] - mean;
+          dd += d * d;
+        }
+      }
+    var = block_sum2(dd, 0.f).x / (float)H;
+  }
+  return make_float2(mean, rsqrtf(var + eps));
+}
+
 __global__ void __launch_bounds__(NORM_THREADS)
 layernorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
                      const bf16* __restrict__ b, bf16* __restrict__ y, int M, int H, float eps) {
@@ -207,26 +240,13 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
   for (long long row = blockIdx.x; row < M; row += gridDim.x) {
     const bf16* xr = x + row * H;
     float cache[NORM_MAXCH][8];
-    float s = 0.f, ss = 0.f;
 #pragma unroll
     for (int ci = 0; ci < NORM_MAXCH; ++ci) {
       const int c = threadIdx.x + ci * NORM_THREADS;
-      if (c < nch) {
-        load8(xr + c * 8, cache[ci]);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { s += cache[ci][j]; ss += cache[ci][j] * cache[ci][j]; }
-      }
+      if (c < nch) load8(xr + c * 8, cache[ci]);
     }
-    for (int c = threadIdx.x + NORM_MAXCH * NORM_THREADS; c < nch; c += NORM_THREADS) {
-      float v[8];
-      load8(xr + c * 8, v);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { s += v[j]; ss += v[j] * v[j]; }
-    }
-    const float2 tot = block_sum2(s, ss);
-    const float mean = tot.x / (float)H;
-    const float var = fmaxf(tot.y / (float)H - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + eps);
+    const float2 st = layernorm_stats(cache, nch, H, eps);
+    const float mean = st.x, rstd = st.y;
     bf16* yr = y + row * H;
 #pragma unroll
     for (int ci = 0; ci < NORM_MAXCH; ++ci) {
@@ -239,15 +259,6 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
         for (int j = 0; j < 8; ++j) o[j] = (cache[ci][j] - mean) * rstd * wv[j] + bv[j];
         store8(yr + c * 8, o);
       }
-    }
-    for (int c = threadIdx.x + NORM_MAXCH * NORM_THREADS; c < nch; c += NORM_THREADS) {
-      float v[8], wv[8], bv[8];
-      load8(xr + c * 8, v);
-      load8(w + c * 8, wv);
-      load8(b + c * 8, bv);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = (v[j] - mean) * rstd * wv[j] + bv[j];
-      store8(yr + c * 8, v);
     }
   }
 }
@@ -270,19 +281,13 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
     const bf16* xr = x + row * H;
     const bf16* dyr = dy + row * H;
     float xv[NORM_MAXCH][8], g[NORM_MAXCH][8];
-    float s = 0.f, ss = 0.f;
 #pragma unroll
     for (int ci = 0; ci < NORM_MAXCH; ++ci) {
       const int c = threadIdx.x + ci * NORM_THREADS;
-      if (c >= nch) continue;
-      load8(xr + c * 8, xv[ci]);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { s += xv[ci][j]; ss += xv[ci][j] * xv[ci][j]; }
+      if (c < nch) load8(xr + c * 8, xv[ci]);
     }
-    const float2 tot = block_sum2(s, ss);
-    const float mean = tot.x / (float)H;
-    const float var = fmaxf(tot.y / (float)H - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + eps);
+    const float2 st = layernorm_stats(xv, nch, H, eps);
+    const float mean = st.x, rstd = st.y;
     float sg = 0.f, sgx = 0.f;
 #pragma unroll
     for (int ci = 0; ci < NORM_MAXCH; ++ci) {
@@ -1292,7 +1297,8 @@ extern "C" int rlaifv_rmsnorm_bwd_partials(void) { return num_sms() * 2; }
 extern "C" int rlaifv_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd,
                                   const void* dres, void* dx, void* dw, int dw_accumulate,
                                   float* workspace, int M, int H, void* stream) {
-  B200_REQUIRE(H % 8 == 0 && H <= NORM_THREADS * 8 * NORM_MAXCH, "rmsnorm_bwd: H=%d unsupported", H);
+  B200_REQUIRE(H % 8 == 0 && H <= NORM_THREADS * 8 * NORM_MAXCH && M > 0, "rmsnorm_bwd: shape [%d,%d] unsupported", M,
+               H);
   int grid = num_sms() * 2;
   if (grid > (M + 1) / 2) grid = (M + 1) / 2;
   rmsnorm_bwd_kernel<<<grid, NORM_THREADS, 0, ST>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, rstd,
@@ -1305,7 +1311,8 @@ extern "C" int rlaifv_rmsnorm_bwd(const void* dy, const void* x, const void* w, 
 
 extern "C" int rlaifv_layernorm_fwd(const void* x, const void* w, const void* b, void* y, int M, int H,
                                     float eps, void* stream) {
-  B200_REQUIRE(H % 8 == 0 && M > 0, "layernorm_fwd: bad shape");
+  B200_REQUIRE(H % 8 == 0 && H <= NORM_THREADS * 8 * NORM_MAXCH && M > 0, "layernorm_fwd: shape [%d,%d] unsupported", M,
+               H);
   const int grid = M < num_sms() * 8 ? M : num_sms() * 8;
   layernorm_fwd_kernel<<<grid, NORM_THREADS, 0, ST>>>((const bf16*)x, (const bf16*)w, (const bf16*)b,
                                                      (bf16*)y, M, H, eps);
