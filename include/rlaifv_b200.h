@@ -176,6 +176,7 @@ int rlaifv_dropout_rows_bwd_add(void* dx, const void* g, const int* rows, long l
 int rlaifv_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd_or_null, int M, int H, float eps,
                        void* stream);
 int rlaifv_rmsnorm_bwd_partials(void); /* rows of the fp32 [partials][H] workspace rmsnorm_bwd needs */
+/* H % 8 == 0 and H <= 6144 (up to LLaVA-1.5-13B's 5120) */
 int rlaifv_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd,
                        const void* dres_or_null, void* dx, void* dw, int dw_accumulate, float* workspace,
                        int M, int H, void* stream);

@@ -100,6 +100,8 @@ rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, bf16*
 // RMSNorm backward. xhat = x*rstd, g = w*dy:
 //   dx = rstd * (g - xhat * mean(g*xhat))  (+ dres if given);  dw[h] += sum_rows dy*xhat
 // dw is accumulated per CTA in registers over its rows and written to dw_partial[grid][H] (fp32).
+// NCH 8-element chunks per thread are register-cached, so H <= NORM_THREADS * 8 * NCH.
+template <int NCH>
 __global__ void __launch_bounds__(NORM_THREADS)
 rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
                    const bf16* __restrict__ w, const float* __restrict__ rstd_in,
@@ -109,19 +111,19 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
   // bytes in flight per CTA and halves the number of block-wide synchronisations (one row per pass ran at 45 % of the
   // copy peak: 2 CTAs/SM x 24 KB in flight, serialised by two __syncthreads per row).
   const int nch = H >> 3;
-  float dwacc[NORM_MAXCH][8];
+  float dwacc[NCH][8];
 #pragma unroll
-  for (int i = 0; i < NORM_MAXCH; ++i)
+  for (int i = 0; i < NCH; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) dwacc[i][j] = 0.f;
   for (long long row0 = 2LL * blockIdx.x; row0 < M; row0 += 2LL * gridDim.x) {
     const bool two = row0 + 1 < M;
     const long long rows[2] = {row0, two ? row0 + 1 : row0};
     const float rstd[2] = {rstd_in[rows[0]], rstd_in[rows[1]]};
-    float xh[2][NORM_MAXCH][8], g[2][NORM_MAXCH][8];
+    float xh[2][NCH][8], g[2][NCH][8];
     float dot[2] = {0.f, 0.f};
 #pragma unroll
-    for (int ci = 0; ci < NORM_MAXCH; ++ci) {
+    for (int ci = 0; ci < NCH; ++ci) {
       const int c = threadIdx.x + ci * NORM_THREADS;
       if (c >= nch) continue;
       float wv[8], xv[2][8], dv[2][8];
@@ -149,7 +151,7 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
     for (int u = 0; u < 2; ++u) {
       if (u == 1 && !two) break;
 #pragma unroll
-      for (int ci = 0; ci < NORM_MAXCH; ++ci) {
+      for (int ci = 0; ci < NCH; ++ci) {
         const int c = threadIdx.x + ci * NORM_THREADS;
         if (c >= nch) continue;
         float o[8];
@@ -166,7 +168,7 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
     }
   }
 #pragma unroll
-  for (int ci = 0; ci < NORM_MAXCH; ++ci) {
+  for (int ci = 0; ci < NCH; ++ci) {
     const int c = threadIdx.x + ci * NORM_THREADS;
     if (c >= nch) continue;
     float* dst = dw_partial + (long long)blockIdx.x * H + c * 8;
@@ -1297,12 +1299,18 @@ extern "C" int rlaifv_rmsnorm_bwd_partials(void) { return num_sms() * 2; }
 extern "C" int rlaifv_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd,
                                   const void* dres, void* dx, void* dw, int dw_accumulate,
                                   float* workspace, int M, int H, void* stream) {
-  B200_REQUIRE(H % 8 == 0 && H <= NORM_THREADS * 8 * NORM_MAXCH && M > 0, "rmsnorm_bwd: shape [%d,%d] unsupported", M,
-               H);
+  // Two chunks per thread cover H <= 4096 (LLaVA-1.5-7B, Mistral-7B); three cover H <= 6144 (LLaVA-1.5-13B: 5120).
+  B200_REQUIRE(H % 8 == 0 && H <= NORM_THREADS * 8 * (NORM_MAXCH + 1) && M > 0,
+               "rmsnorm_bwd: shape [%d,%d] unsupported", M, H);
   int grid = num_sms() * 2;
   if (grid > (M + 1) / 2) grid = (M + 1) / 2;
-  rmsnorm_bwd_kernel<<<grid, NORM_THREADS, 0, ST>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w, rstd,
-                                                   (const bf16*)dres, (bf16*)dx, workspace, M, H);
+  if (H <= NORM_THREADS * 8 * NORM_MAXCH)
+    rmsnorm_bwd_kernel<NORM_MAXCH><<<grid, NORM_THREADS, 0, ST>>>((const bf16*)dy, (const bf16*)x, (const bf16*)w,
+                                                                 rstd, (const bf16*)dres, (bf16*)dx, workspace, M, H);
+  else
+    rmsnorm_bwd_kernel<NORM_MAXCH + 1><<<grid, NORM_THREADS, 0, ST>>>((const bf16*)dy, (const bf16*)x,
+                                                                     (const bf16*)w, rstd, (const bf16*)dres,
+                                                                     (bf16*)dx, workspace, M, H);
   B200_CHECK_CUDA(cudaGetLastError());
   reduce_partials_kernel<<<(H + 31) / 32, 256, 0, ST>>>(workspace, grid, H, (bf16*)dw, dw_accumulate);
   B200_CHECK_CUDA(cudaGetLastError());

@@ -1,11 +1,12 @@
-"""Time the frozen-base GEMMs of one LLaVA-1.5-7B LoRA-DPO step shape by shape, against cuBLAS on the same card.
+"""Time the frozen-base GEMMs of one LLaVA-1.5 LoRA-DPO step shape by shape, against cuBLAS on the same card.
 
-    python tools/gemm_step_shapes.py --out DIR [--stalls] [--min-seconds 1.0]
+    python tools/gemm_step_shapes.py --out DIR [--dims 7b|13b] [--stalls] [--min-seconds 1.0]
 
 The calls are recorded, not re-typed: one training step of a one-decoder-layer LoRA(r=64) policy at the benchmark's
 batch (8 pairs, micro-batches of 4, T = 1135) runs with ops.gemm, ops.gemm_dual and ops.gemm_swiglu_bwd wrapped, so
-every shape keeps its operand layouts, epilogue and LoRA second source. A decoder layer's calls repeat 32 times per
-step. Per frozen-base shape, in one process, alternating between the variants:
+every shape keeps its operand layouts, epilogue and LoRA second source. A decoder layer's calls repeat once per layer
+per step: 32 times for LLaVA-1.5-7B (--dims 7b, hidden 4096, ffn 11008), 40 times for LLaVA-1.5-13B (--dims 13b,
+hidden 5120, ffn 13824). Per frozen-base shape, in one process, alternating between the variants:
 
   ours           the shipped path, automatic tile choice
   ours-register  the same launch with the register epilogue (rlaifv_gemm_set_tuning(0, 2)): threads store C straight
@@ -35,26 +36,26 @@ import time
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
-LAYERS = 32                 # LLaVA-1.5-7B decoder layers: the recorded one-layer calls repeat this often per step
+# decoder widths and layers of each model: the recorded one-layer calls repeat `layers` times per step
+DIMS = {"7b": dict(hidden_size=4096, intermediate_size=11008, num_heads=32, layers=32),
+        "13b": dict(hidden_size=5120, intermediate_size=13824, num_heads=40, layers=40)}
 PAIRS, MICRO_PAIRS = 8, 4   # bench.py: pairs per step and per micro-batch
 STALL_FIELDS = ("ctas", "tiles", "cons_total", "cons_full_wait", "cons_epilogue", "prod_total", "prod_empty_wait")
 
-# names of the frozen-base shapes: (function, N, K) -> name; N / K are the launch's output columns / first-source depth
-SHAPE_NAMES = {
-    ("gemm_dual", 12288, 4096): "qkv forward",
-    ("gemm_dual", 4096, 4096, False): "o forward",
-    ("gemm_dual", 22016, 4096): "gate|up forward",
-    ("gemm_dual", 4096, 11008): "down forward",
-    ("gemm_swiglu_bwd", 11008, 4096): "down dgrad (SwiGLU bwd)",
-    ("gemm_dual", 4096, 22016): "gate|up dgrad",
-    ("gemm_dual", 4096, 4096, True): "o dgrad",
-    ("gemm_dual", 4096, 12288): "qkv dgrad",
-}
+
+def shape_names(H, F):
+    """Names of the frozen-base shapes: (function, N, K) -> name; N / K are the launch's output columns / first-source
+    depth. The two H x H launches are told apart by the layout of B."""
+    return {("gemm_dual", 3 * H, H): "qkv forward", ("gemm_dual", H, H, False): "o forward",
+            ("gemm_dual", 2 * F, H): "gate|up forward", ("gemm_dual", H, F): "down forward",
+            ("gemm_swiglu_bwd", F, H): "down dgrad (SwiGLU bwd)", ("gemm_dual", H, 2 * F): "gate|up dgrad",
+            ("gemm_dual", H, H, True): "o dgrad", ("gemm_dual", H, 3 * H): "qkv dgrad"}
 
 
 def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--out", required=True, help="output directory (JSON, stall-accounting build)")
+    ap.add_argument("--dims", choices=sorted(DIMS), default="7b", help="decoder widths: LLaVA-1.5-7B or -13B")
     ap.add_argument("--min-seconds", type=float, default=1.0, help="timed work per variant and shape")
     ap.add_argument("--adapter-seconds", type=float, default=0.2, help="timed work per adapter GEMM shape")
     ap.add_argument("--stalls", action="store_true", help="build and run the stall-accounting variant too")
@@ -134,14 +135,16 @@ def card_info():
     return info
 
 
-def record_step_calls():
+def record_step_calls(dims):
     """One LoRA-DPO training step of a one-layer policy at the benchmark's batch: every GEMM call with its tensors."""
     import torch
     import bench
     from rlaifv_b200 import ops
     from rlaifv_b200.engine import DPOStepEngine
     from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
-    policy = LlavaDPOPolicy(LlavaDims(num_layers=1), torch.device("cuda", 0), seed=0)
+    policy = LlavaDPOPolicy(LlavaDims(num_layers=1, hidden_size=dims["hidden_size"],
+                                      intermediate_size=dims["intermediate_size"], num_heads=dims["num_heads"]),
+                            torch.device("cuda", 0), seed=0)
     policy.enable_lora(r=64, alpha=16)
     engine = DPOStepEngine(policy, lr=1e-5, weight_decay=0.01, total_steps=2672, micro_pairs=MICRO_PAIRS)
     hb = bench.synthetic_batch(0, 0, PAIRS)
@@ -196,11 +199,12 @@ def describe(name, a, kw, r):
     return (name, t_sig, kw_sig), d
 
 
-def shape_name(d):
+def shape_name(d, dims):
+    H = dims["hidden_size"]
     key = (d["fn"], d["N"], d["K"])
-    if d["fn"] == "gemm_dual" and d["N"] == d["K"] == 4096:
+    if d["fn"] == "gemm_dual" and d["N"] == d["K"] == H:
         key = key + (d["B"] == "MN",)
-    return SHAPE_NAMES.get(key)
+    return shape_names(H, dims["intermediate_size"]).get(key)
 
 
 def is_adapter(d, r=64):
@@ -243,7 +247,8 @@ def main(argv=None):
     args = parse_args(argv)
     os.makedirs(args.out, exist_ok=True)
     stall_so = None
-    result = {"tag": args.tag, "group_m": args.group_m, "l2": args.l2}
+    dims = DIMS[args.dims]
+    result = {"tag": args.tag, "group_m": args.group_m, "l2": args.l2, "dims": args.dims}
     if args.stalls:
         stall_so, spills = build_stall_library(args.out)
         result["stall_build"] = {"library": os.path.relpath(stall_so, args.out), "ptxas_spill_lines": spills}
@@ -266,7 +271,7 @@ def main(argv=None):
         L.rlaifv_gemm_set_tuning(args.group_m, 0)
         L.rlaifv_gemm_set_l2(args.l2)
 
-    calls, keep = record_step_calls()
+    calls, keep = record_step_calls(dims)
     uniq = {}
     for name, a, kw, r in calls:
         sig, d = describe(name, a, kw, r)
@@ -307,14 +312,14 @@ def main(argv=None):
     ad_calls = 0
     try:   # the sampler is a child process: stop it whatever happens to the timings
         for d, call, count in frozen:
-            per_step = count * LAYERS              # the recorded step already holds both micro-batches
+            per_step = count * dims["layers"]      # the recorded step already holds both micro-batches
             v = {"ours": ours_fn(call), "ours-register": debug_fn(call, 2), "ours-mainloop": debug_fn(call, 1)}
             if not args.no_cublas:
                 v["cublas"] = cublas_fn(call, d)
             ms = time_variants(v, args.min_seconds)
             fl = 2.0 * d["M"] * d["N"] * (d["K"] + d["K2"])
             fl_cublas = 2.0 * d["M"] * d["N"] * d["K"]
-            row = dict(d, name=shape_name(d), calls_per_step=per_step, gflop=fl / 1e9)
+            row = dict(d, name=shape_name(d, dims), calls_per_step=per_step, gflop=fl / 1e9)
             for n, t in ms.items():
                 f = fl_cublas if n == "cublas" else fl
                 row[n] = {"ms_per_call": t, "ms_per_step": t * per_step, "tflops": f / (t * 1e-3) / 1e12}
@@ -326,7 +331,7 @@ def main(argv=None):
                   d["A"], d["B"], d["epilogue"], per_step) +
                   "  ".join(" %s %.3f ms %.0f TF/s" % (n, row[n]["ms_per_call"], row[n]["tflops"]) for n in ms), flush=True)
         for d, call, count in adapters:
-            per_step = count * LAYERS
+            per_step = count * dims["layers"]
             t = time_variants({"ours": ours_fn(call)}, args.adapter_seconds, rounds=1)["ours"]
             ad_ms += t * per_step
             ad_fl += 2.0 * d["M"] * d["N"] * d["K"] * per_step
