@@ -334,9 +334,9 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
 }
 
 // y[r] = bf16(x[r] + t[r % P])  — the resampler's position-embedding adds (resampler.py:158-161): the table t
-// ([P][H], frozen sin-cos embedding) is shared by every image of the batch.
-__global__ void add_rows_bcast_kernel(const bf16* __restrict__ x, const bf16* __restrict__ t, bf16* __restrict__ y,
-                                      long long M, int P, int H) {
+// ([P][H], frozen sin-cos embedding) is shared by every image of the batch. y may alias x: the EVA tower's cls
+// gradient and the resampler's query gradient are accumulated in place (out = x), so x and y are not __restrict__.
+__global__ void add_rows_bcast_kernel(const bf16* x, const bf16* __restrict__ t, bf16* y, long long M, int P, int H) {
   const int nch = H >> 3;
   const long long total = M * nch;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
