@@ -159,6 +159,22 @@ int rlaifv_attention_varlen_bwd(const void* q, const void* k, const void* v, lon
                                 long long ld_dq, void* dk, void* dv, long long ld_dkv, float* delta_ws, const int* cu,
                                 int nseq, int max_len, long long n_rows, int n_heads, int n_kv_heads, int head_dim,
                                 float scale, void* stream);
+/* The same with borrowed prefixes: two sequences whose inputs agree below a position keep one copy of those rows.
+ * pos0 and partner are int32 [nseq] HOST arrays (nseq <= 64). Sequence s's rows [cu[s], cu[s+1]) hold positions
+ * pos0[s] .. pos0[s] + len_s - 1, pos0[s] a multiple of 128; with pos0[s] > 0 its positions t < pos0[s] are the rows
+ * cu[partner[s]] + t of its lender (pos0 0, partner s, at least pos0[s] rows). partner -1 = neither lends nor borrows.
+ * O, LSE, dQ and the dK/dV of a borrower's rows get the bits the fixed-length kernels give the sequence padded; a
+ * lender's rows below its borrower's pos0 get the sum of both sequences' dK/dV. */
+int rlaifv_attention_varlen_prefix_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out,
+                                       long long ld_out, float* lse, const int* cu, const int* pos0,
+                                       const int* partner, int nseq, int max_len, long long n_rows, int n_heads,
+                                       int n_kv_heads, int head_dim, float scale, void* stream);
+int rlaifv_attention_varlen_prefix_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out,
+                                       long long ld_out, const void* d_out, long long ld_dout, const float* lse,
+                                       void* dq, long long ld_dq, void* dk, void* dv, long long ld_dkv,
+                                       float* delta_ws, const int* cu, const int* pos0, const int* partner, int nseq,
+                                       int max_len, long long n_rows, int n_heads, int n_kv_heads, int head_dim,
+                                       float scale, void* stream);
 /* RoPE on the fused [q | k | v] rows with the position of row m taken from pos[m] (int32 [M], device); the backward
  * rotates the q block (split attention backward) and the k block in place. */
 int rlaifv_rope_pos_fwd(void* qkv, const void* cos_tab, const void* sin_tab, const int* pos, long long M, int n_heads,

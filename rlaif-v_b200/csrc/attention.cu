@@ -773,13 +773,31 @@ extern "C" int rlaifv_cross_attention_bwd(const void* q, long long ld_q, const v
 // kernels above on the same sequence padded to any length: the results at rows < len_s are the same bits. A tile's
 // rows past len_s are the next sequence's (or TMA zero-fill past the last row): causality hides them from valid
 // queries in the forward and the dQ kernel; the dK/dV kernel, where they come after the key, masks them explicitly.
+//
+// Borrowed prefixes (PREFIX = true, the attention_varlen_prefix_* entry points): sequence s's own rows hold positions
+// p0 = pos0[s] .. p0 + len_s - 1, and with p0 > 0 its positions below p0 are rows of its lender partner[s] (two
+// sequences with identical inputs below p0 hold identical rows there, so one copy serves both). p0 is a multiple of
+// 128: every own query row sees the key partition and chunk order of the fixed-length kernels on the sequence padded
+// to any length, so O, LSE, dQ and the dK/dV of own rows are those kernels' bits. A lender's key tile below its
+// borrower's p0 streams the lender's Q / dO chunks, then the borrower's, into one accumulator: its dK/dV is the sum
+// of both copies' gradients. LSE and delta keep the [n_heads][len_s] blocks of own rows.
 namespace b200 {
 
+constexpr int PREFIX_MAX_SEQ = 64;
+template <bool PREFIX>
+struct PrefixMap {
+  int pos0[PREFIX_MAX_SEQ];
+  int partner[PREFIX_MAX_SEQ];
+};
+template <>
+struct PrefixMap<false> {};
+
+template <bool PREFIX>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_varlen_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                             const __grid_constant__ CUtensorMap tmV, bf16* __restrict__ out, long long ld_out,
                             float* __restrict__ lse_out, const int* __restrict__ cu, int n_heads, int kv_group,
-                            float scale) {
+                            float scale, const __grid_constant__ PrefixMap<PREFIX> pm) {
   constexpr int D = 128;
   using Cfg = AttFwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
@@ -794,12 +812,18 @@ attention_varlen_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __gri
   const int row0 = cu[seq], len = cu[seq + 1] - row0;
   const int num_q_tiles = (len + ATT_BQ - 1) / ATT_BQ;
   if ((int)blockIdx.x >= num_q_tiles) return;             // the grid is sized for the longest sequence
+  int p0 = 0, lrow0 = row0;                               // first own position; the lender's row of position 0
+  if constexpr (PREFIX) {
+    p0 = pm.pos0[seq];
+    if (p0 > 0) lrow0 = cu[pm.partner[seq]];
+  }
+  const int end = p0 + len;                               // one past the last position
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const int q_tile = num_q_tiles - 1 - blockIdx.x;        // heavy (late) tiles first
   const int head = blockIdx.y;
   const int kv_head = head / kv_group;
-  const int q0 = q_tile * ATT_BQ;
-  const int n_kv = min(num_q_tiles, (q0 + ATT_BQ + ATT_BKV - 1) / ATT_BKV);
+  const int q0 = p0 + q_tile * ATT_BQ;
+  const int n_kv = min(num_q_tiles + p0 / ATT_BKV, (q0 + ATT_BQ + ATT_BKV - 1) / ATT_BKV);
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
@@ -815,17 +839,19 @@ attention_varlen_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __gri
       tma_prefetch_desc(&tmV);
       mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
 #pragma unroll
-      for (int a = 0; a < D / 64; ++a) tma_load_2d(smem + a * Cfg::Q_ATOM, &tmQ, q_full, head * D + a * 64, row0 + q0);
+      for (int a = 0; a < D / 64; ++a)
+        tma_load_2d(smem + a * Cfg::Q_ATOM, &tmQ, q_full, head * D + a * 64, row0 - p0 + q0);
       for (int j = 0; j < n_kv; ++j) {
         const int s = j % ATT_STAGES;
         if (j >= ATT_STAGES) mbar_wait(&kv_empty[s], ((j / ATT_STAGES) - 1) & 1);
         mbar_arrive_expect_tx(&kv_full[s], 2 * Cfg::KV_BYTES);
+        const int kv_row = (PREFIX && j * ATT_BKV < p0 ? lrow0 : row0 - p0) + j * ATT_BKV;
 #pragma unroll
         for (int a = 0; a < D / 64; ++a) {
           tma_load_2d(smem + Cfg::OFF_K + s * Cfg::KV_BYTES + a * Cfg::KV_ATOM, &tmK, &kv_full[s],
-                      kv_head * D + a * 64, row0 + j * ATT_BKV);
+                      kv_head * D + a * 64, kv_row);
           tma_load_2d(smem + Cfg::OFF_V + s * Cfg::KV_BYTES + a * Cfg::KV_ATOM, &tmV, &kv_full[s],
-                      kv_head * D + a * 64, row0 + j * ATT_BKV);
+                      kv_head * D + a * 64, kv_row);
         }
       }
     }
@@ -851,13 +877,13 @@ attention_varlen_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __gri
       wgmma_wait<0>();
       reg_fence(sv);
       const int kv0 = j * ATT_BKV;
-      if (kv0 + ATT_BKV > len || kv0 + ATT_BKV - 1 > q0 + wg * 64) {
+      if (kv0 + ATT_BKV > end || kv0 + ATT_BKV - 1 > q0 + wg * 64) {
 #pragma unroll
         for (int i = 0; i < 16; ++i)
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const int kv = kv0 + 8 * i + fp.c0 + (e & 1);
-            if (kv >= len || kv > qr[e >> 1]) sv[4 * i + e] = -INFINITY;
+            if (kv >= end || kv > qr[e >> 1]) sv[4 * i + e] = -INFINITY;
           }
       }
       float mx[2] = {-INFINITY, -INFINITY};
@@ -907,13 +933,14 @@ attention_varlen_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __gri
       l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
       l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
       const int q = qr[h];
-      if (q >= len) continue;
+      if (q >= end) continue;
       const float inv = 1.f / l[h];
-      bf16* o_row = out + ((long long)row0 + q) * ld_out + head * D + fp.c0;
+      bf16* o_row = out + ((long long)row0 - p0 + q) * ld_out + head * D + fp.c0;
 #pragma unroll
       for (int i = 0; i < D / 8; ++i)
         *reinterpret_cast<uint32_t*>(o_row + 8 * i) = pack_bf16(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
-      if (fp.c0 == 0) lse_out[(long long)n_heads * row0 + (long long)head * len + q] = (m_run[h] + log2f(l[h])) * LN2;
+      if (fp.c0 == 0)
+        lse_out[(long long)n_heads * row0 + (long long)head * len + q - p0] = (m_run[h] + log2f(l[h])) * LN2;
     }
   }
 }
@@ -965,12 +992,21 @@ __global__ void attention_varlen_delta_kernel(const bf16* __restrict__ o, long l
   }
 }
 
-// one pass of attention_bwd_dkv_kernel over packed rows; query rows >= len are masked (P = dS = 0)
-template <bool DK>
+// The query chunks a dK/dV tile streams, per query head: n_own chunks of its own sequence from position c_first * 64
+// (LSE / delta block at blk0, len rows from position p0), then, for a lender's tile below its borrower's first own
+// position, the borrower's n_c - n_own chunks from position b_p0 (block b_blk, b_len rows).
+struct DkvChunks {
+  int n_own, p0, b_p0, b_len;
+  long long b_blk;
+};
+
+// one pass of attention_bwd_dkv_kernel over packed rows; query positions past the sequence's end are masked
+// (P = dS = 0)
+template <bool DK, bool PREFIX>
 __device__ __forceinline__ void varlen_dkv_pass(uint8_t* smem, uint64_t* c_full, uint64_t* c_empty, int it0, int n_it,
                                                 int n_c, int c_first, int kv_head, int kv_group, long long blk0, int len,
-                                                const int (&kvr)[2], uint32_t k_addr, uint32_t v_addr, float c,
-                                                float scale, const float* __restrict__ lse,
+                                                const DkvChunks& ch, const int (&kvr)[2], uint32_t k_addr,
+                                                uint32_t v_addr, float c, float scale, const float* __restrict__ lse,
                                                 const float* __restrict__ delta, float (&acc)[BWD_D / 2]) {
   using Cfg = AttBwdCfg;
   const FragPos fp = frag_pos();
@@ -978,9 +1014,22 @@ __device__ __forceinline__ void varlen_dkv_pass(uint8_t* smem, uint64_t* c_full,
   for (int i = 0; i < BWD_D / 2; ++i) acc[i] = 0.f;
   for (int it = 0; it < n_it; ++it) {
     const int ii = it0 + it, s = ii % ATT_STAGES;
-    const int qc0 = (c_first + it % n_c) * BWD_C;
+    const int k = it % n_c;
     const int head = kv_head * kv_group + it / n_c;
-    const long long base = blk0 + (long long)head * len;
+    int qc0 = (c_first + k) * BWD_C;
+    long long base = blk0 + (long long)head * len;        // LSE / delta of position q at base + q - p0
+    int p0 = 0, len_q = len;
+    if constexpr (PREFIX) {
+      p0 = ch.p0;
+      if (k >= ch.n_own) {
+        qc0 = ch.b_p0 + (k - ch.n_own) * BWD_C;
+        base = ch.b_blk + (long long)head * ch.b_len;
+        p0 = ch.b_p0;
+        len_q = ch.b_len;
+      }
+    }
+    base -= p0;
+    const int end = p0 + len_q;
     const uint32_t q_addr = smem_u32(smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES);
     const uint32_t do_addr = q_addr + Cfg::CHUNK_BYTES;
     mbar_wait(&c_full[s], (ii / ATT_STAGES) & 1);
@@ -995,17 +1044,17 @@ __device__ __forceinline__ void varlen_dkv_pass(uint8_t* smem, uint64_t* c_full,
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int q = qc0 + 8 * i + fp.c0;
-      const float l0 = q < len ? lse[base + q] * LOG2E : INFINITY, l1 = q + 1 < len ? lse[base + q + 1] * LOG2E : INFINITY;
+      const float l0 = q < end ? lse[base + q] * LOG2E : INFINITY, l1 = q + 1 < end ? lse[base + q + 1] * LOG2E : INFINITY;
       float d0 = 0.f, d1 = 0.f;
       if (DK) {
-        d0 = q < len ? delta[base + q] : 0.f;
-        d1 = q + 1 < len ? delta[base + q + 1] : 0.f;
+        d0 = q < end ? delta[base + q] : 0.f;
+        d1 = q + 1 < end ? delta[base + q + 1] : 0.f;
       }
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int qq = q + (e & 1);
-        // rows >= len belong to the next sequence (causality does not hide them: they come after the key)
-        const bool masked = kvr[e >> 1] > qq || qq >= len;
+        // rows past the end belong to the next sequence (causality does not hide them: they come after the key)
+        const bool masked = kvr[e >> 1] > qq || qq >= end;
         const float p = masked ? 0.f : fast_exp2(st[4 * i + e] * c - ((e & 1) ? l1 : l0));
         st[4 * i + e] = masked ? 0.f : DK ? p * (dpt[4 * i + e] - ((e & 1) ? d1 : d0)) * scale : p;
       }
@@ -1022,12 +1071,13 @@ __device__ __forceinline__ void varlen_dkv_pass(uint8_t* smem, uint64_t* c_full,
   }
 }
 
+template <bool PREFIX>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_varlen_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
                                 const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dk,
                                 bf16* __restrict__ dv, long long ld_dkv, const int* __restrict__ cu, int n_heads,
-                                int kv_group, float scale) {
+                                int kv_group, float scale, const __grid_constant__ PrefixMap<PREFIX> pm) {
   using Cfg = AttBwdCfg;
   constexpr int D = BWD_D;
   extern __shared__ uint8_t smem_raw[];
@@ -1040,12 +1090,26 @@ attention_varlen_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const _
 
   const int seq = blockIdx.z;
   const int row0 = cu[seq], len = cu[seq + 1] - row0;
-  const int kv0 = blockIdx.x * 128;
-  if (kv0 >= len) return;
+  if ((int)blockIdx.x * 128 >= len) return;
+  DkvChunks ch{0, 0, 0, 0, 0};
+  int b_row0 = 0;                                             // the borrower's first own row
+  if constexpr (PREFIX) ch.p0 = pm.pos0[seq];
+  const int kv0 = ch.p0 + blockIdx.x * 128;
   const int warp = threadIdx.x >> 5, wg = warp >> 2;
   const int kv_head = blockIdx.y;
   const int c_first = kv0 / BWD_C;                            // chunks holding a q >= kv0
-  const int n_c = (len + BWD_C - 1) / BWD_C - c_first;        // >= 1
+  ch.n_own = (ch.p0 + len + BWD_C - 1) / BWD_C - c_first;     // >= 1
+  int n_c = ch.n_own;
+  if constexpr (PREFIX) {
+    const int b = pm.partner[seq];
+    if (ch.p0 == 0 && b >= 0 && kv0 < pm.pos0[b]) {           // a lender's key tile below its borrower's own rows
+      b_row0 = cu[b];
+      ch.b_p0 = pm.pos0[b];
+      ch.b_len = cu[b + 1] - b_row0;
+      ch.b_blk = (long long)n_heads * b_row0;
+      n_c += (ch.b_len + BWD_C - 1) / BWD_C;
+    }
+  }
   const int n_it = n_c * kv_group;
   const long long blk0 = (long long)n_heads * row0;
 
@@ -1061,19 +1125,24 @@ attention_varlen_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const _
       tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
       mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
       for (int a = 0; a < 2; ++a) {
-        tma_load_2d(smem + a * Cfg::TILE_ATOM, &tmK, kv_full, kv_head * D + a * 64, row0 + kv0);
-        tma_load_2d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmV, kv_full, kv_head * D + a * 64, row0 + kv0);
+        tma_load_2d(smem + a * Cfg::TILE_ATOM, &tmK, kv_full, kv_head * D + a * 64, row0 - ch.p0 + kv0);
+        tma_load_2d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmV, kv_full, kv_head * D + a * 64, row0 - ch.p0 + kv0);
       }
       for (int ii = 0; ii < 2 * n_it; ++ii) {
         const int it = ii % n_it, s = ii % ATT_STAGES;
         if (ii >= ATT_STAGES) mbar_wait(&c_empty[s], ((ii / ATT_STAGES) - 1) & 1);
         const int qc0 = (c_first + it % n_c) * BWD_C;
         const int head = kv_head * kv_group + it / n_c;
+        int q_row = row0 + qc0;
+        if constexpr (PREFIX) {
+          const int k = it % n_c;
+          q_row = k >= ch.n_own ? b_row0 + (k - ch.n_own) * BWD_C : row0 - ch.p0 + qc0;
+        }
         uint8_t* dst = smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES;
         mbar_arrive_expect_tx(&c_full[s], 2 * Cfg::CHUNK_BYTES);
         for (int a = 0; a < 2; ++a) {
-          tma_load_2d(dst + a * Cfg::CHUNK_ATOM, &tmQ, &c_full[s], head * D + a * 64, row0 + qc0);
-          tma_load_2d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmDO, &c_full[s], head * D + a * 64, row0 + qc0);
+          tma_load_2d(dst + a * Cfg::CHUNK_ATOM, &tmQ, &c_full[s], head * D + a * 64, q_row);
+          tma_load_2d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmDO, &c_full[s], head * D + a * 64, q_row);
         }
       }
     }
@@ -1088,17 +1157,17 @@ attention_varlen_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const _
 #pragma unroll 1
     for (int pass = 0; pass < 2; ++pass) {
       if (pass == 0)
-        varlen_dkv_pass<false>(smem, c_full, c_empty, 0, n_it, n_c, c_first, kv_head, kv_group, blk0, len, kvr, k_addr,
-                               v_addr, c, scale, lse, delta, acc);
+        varlen_dkv_pass<false, PREFIX>(smem, c_full, c_empty, 0, n_it, n_c, c_first, kv_head, kv_group, blk0, len, ch,
+                                       kvr, k_addr, v_addr, c, scale, lse, delta, acc);
       else
-        varlen_dkv_pass<true>(smem, c_full, c_empty, n_it, n_it, n_c, c_first, kv_head, kv_group, blk0, len, kvr,
-                              k_addr, v_addr, c, scale, lse, delta, acc);
+        varlen_dkv_pass<true, PREFIX>(smem, c_full, c_empty, n_it, n_it, n_c, c_first, kv_head, kv_group, blk0, len, ch,
+                                      kvr, k_addr, v_addr, c, scale, lse, delta, acc);
       bf16* dst = pass == 0 ? dv : dk;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int kv = kvr[h];
-        if (kv >= len) continue;
-        bf16* row = dst + ((long long)row0 + kv) * ld_dkv + kv_head * D + fp.c0;
+        if (kv >= ch.p0 + len) continue;
+        bf16* row = dst + ((long long)row0 - ch.p0 + kv) * ld_dkv + kv_head * D + fp.c0;
 #pragma unroll
         for (int i = 0; i < D / 8; ++i)
           *reinterpret_cast<uint32_t*>(row + 8 * i) = pack_bf16(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
@@ -1107,11 +1176,13 @@ attention_varlen_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const _
   }
 }
 
+template <bool PREFIX>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_varlen_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
                                const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dq,
-                               long long ld_dq, const int* __restrict__ cu, int n_heads, int kv_group, float scale) {
+                               long long ld_dq, const int* __restrict__ cu, int n_heads, int kv_group, float scale,
+                               const __grid_constant__ PrefixMap<PREFIX> pm) {
   using Cfg = AttBwdCfg;
   constexpr int D = BWD_D;
   extern __shared__ uint8_t smem_raw[];
@@ -1126,12 +1197,18 @@ attention_varlen_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __
   const int row0 = cu[seq], len = cu[seq + 1] - row0;
   const int num_q_tiles = (len + 127) / 128;
   if ((int)blockIdx.x >= num_q_tiles) return;
+  int p0 = 0, lrow0 = row0;                                   // first own position; the lender's row of position 0
+  if constexpr (PREFIX) {
+    p0 = pm.pos0[seq];
+    if (p0 > 0) lrow0 = cu[pm.partner[seq]];
+  }
+  const int end = p0 + len;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const int q_tile = num_q_tiles - 1 - blockIdx.x;            // heavy (late) tiles first
-  const int q0 = q_tile * 128;
+  const int q0 = p0 + q_tile * 128;
   const int head = blockIdx.y;
   const int kv_head = head / kv_group;
-  const int n_c = min((len + BWD_C - 1) / BWD_C, (q0 + 128 + BWD_C - 1) / BWD_C);
+  const int n_c = min((end + BWD_C - 1) / BWD_C, (q0 + 128 + BWD_C - 1) / BWD_C);
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
@@ -1145,18 +1222,18 @@ attention_varlen_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __
       tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
       mbar_arrive_expect_tx(q_full, 2 * Cfg::TILE_BYTES);
       for (int a = 0; a < 2; ++a) {
-        tma_load_2d(smem + a * Cfg::TILE_ATOM, &tmQ, q_full, head * D + a * 64, row0 + q0);
-        tma_load_2d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmDO, q_full, head * D + a * 64, row0 + q0);
+        tma_load_2d(smem + a * Cfg::TILE_ATOM, &tmQ, q_full, head * D + a * 64, row0 - p0 + q0);
+        tma_load_2d(smem + Cfg::OFF_T1 + a * Cfg::TILE_ATOM, &tmDO, q_full, head * D + a * 64, row0 - p0 + q0);
       }
       for (int j = 0; j < n_c; ++j) {
         const int s = j % ATT_STAGES;
         if (j >= ATT_STAGES) mbar_wait(&c_empty[s], ((j / ATT_STAGES) - 1) & 1);
         uint8_t* dst = smem + Cfg::OFF_C + s * 2 * Cfg::CHUNK_BYTES;
         mbar_arrive_expect_tx(&c_full[s], 2 * Cfg::CHUNK_BYTES);
+        const int kv_row = (PREFIX && j * BWD_C < p0 ? lrow0 : row0 - p0) + j * BWD_C;
         for (int a = 0; a < 2; ++a) {
-          tma_load_2d(dst + a * Cfg::CHUNK_ATOM, &tmK, &c_full[s], kv_head * D + a * 64, row0 + j * BWD_C);
-          tma_load_2d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmV, &c_full[s], kv_head * D + a * 64,
-                      row0 + j * BWD_C);
+          tma_load_2d(dst + a * Cfg::CHUNK_ATOM, &tmK, &c_full[s], kv_head * D + a * 64, kv_row);
+          tma_load_2d(dst + Cfg::CHUNK_BYTES + a * Cfg::CHUNK_ATOM, &tmV, &c_full[s], kv_head * D + a * 64, kv_row);
         }
       }
     }
@@ -1164,12 +1241,12 @@ attention_varlen_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __
     const FragPos fp = frag_pos();
     const int qr[2] = {q0 + wg * 64 + fp.r0, q0 + wg * 64 + fp.r0 + 8};
     const float c = scale * LOG2E;
-    const long long base = (long long)n_heads * row0 + (long long)head * len;
+    const long long base = (long long)n_heads * row0 + (long long)head * len - p0;
     float lse2[2], dl[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      lse2[h] = qr[h] < len ? lse[base + qr[h]] * LOG2E : INFINITY;
-      dl[h] = qr[h] < len ? delta[base + qr[h]] : 0.f;
+      lse2[h] = qr[h] < end ? lse[base + qr[h]] * LOG2E : INFINITY;
+      dl[h] = qr[h] < end ? delta[base + qr[h]] : 0.f;
     }
     float dqacc[D / 2];
 #pragma unroll
@@ -1196,7 +1273,7 @@ attention_varlen_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __
         for (int e = 0; e < 4; ++e) {
           const int kv = j * BWD_C + 8 * i + fp.c0 + (e & 1);
           const int h = e >> 1;
-          const bool masked = kv >= len || kv > qr[h];
+          const bool masked = kv >= end || kv > qr[h];
           const float p = masked ? 0.f : fast_exp2(sv[4 * i + e] * c - lse2[h]);
           dp[4 * i + e] = p * (dp[4 * i + e] - dl[h]) * scale;
         }
@@ -1213,8 +1290,8 @@ attention_varlen_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int q = qr[h];
-      if (q >= len) continue;
-      bf16* row = dq + ((long long)row0 + q) * ld_dq + head * D + fp.c0;
+      if (q >= end) continue;
+      bf16* row = dq + ((long long)row0 - p0 + q) * ld_dq + head * D + fp.c0;
 #pragma unroll
       for (int i = 0; i < D / 8; ++i)
         *reinterpret_cast<uint32_t*>(row + 8 * i) = pack_bf16(dqacc[4 * i + 2 * h], dqacc[4 * i + 2 * h + 1]);
@@ -1240,6 +1317,91 @@ static int varlen_check(const char* who, long long ld_qkv, long long ld_out, voi
   return 0;
 }
 
+// a sequence either lends or borrows, never both, and lends to at most one: pos0 multiples of 128, partner links
+// that pair a borrower (pos0 > 0) with a lender (pos0 == 0) both ways
+static int prefix_check(const char* who, const int* pos0, const int* partner, int nseq, PrefixMap<true>* pm) {
+  B200_REQUIRE(pos0 != nullptr && partner != nullptr, "%s: pos0 / partner missing", who);
+  B200_REQUIRE(nseq <= PREFIX_MAX_SEQ, "%s: %d sequences (at most %d)", who, nseq, PREFIX_MAX_SEQ);
+  for (int s = 0; s < nseq; ++s) {
+    const int p = pos0[s], b = partner[s];
+    B200_REQUIRE(p >= 0 && p % ATT_BKV == 0, "%s: pos0[%d] = %d is not a non-negative multiple of %d", who, s, p,
+                 ATT_BKV);
+    B200_REQUIRE(b >= -1 && b < nseq && b != s, "%s: partner[%d] = %d out of range", who, s, b);
+    B200_REQUIRE(p == 0 || b >= 0, "%s: sequence %d borrows (pos0 %d) without a lender", who, s, p);
+    B200_REQUIRE(b < 0 || (partner[b] == s && (p > 0) != (pos0[b] > 0)),
+                 "%s: sequences %d and %d are not one lender and one borrower of each other", who, s, b);
+    pm->pos0[s] = p;
+    pm->partner[s] = b;
+  }
+  return 0;
+}
+
+template <bool PREFIX>
+static int varlen_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out,
+                      float* lse, const int* cu, int nseq, int max_len, long long n_rows, int n_heads, int n_kv_heads,
+                      int head_dim, float scale, void* stream, const PrefixMap<PREFIX>& pm) {
+  int rc;
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_packed_tmap(&tq, q, ld_qkv, n_rows, n_heads * head_dim, ATT_BQ))) return rc;
+  if ((rc = make_packed_tmap(&tk, k, ld_qkv, n_rows, n_kv_heads * head_dim, ATT_BKV))) return rc;
+  if ((rc = make_packed_tmap(&tv, v, ld_qkv, n_rows, n_kv_heads * head_dim, ATT_BKV))) return rc;
+  auto kern = attention_varlen_fwd_kernel<PREFIX>;
+  B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)AttFwdCfg<128>::SMEM_BYTES));
+  dim3 grid((max_len + ATT_BQ - 1) / ATT_BQ, n_heads, nseq);
+  kern<<<grid, ATT_THREADS, AttFwdCfg<128>::SMEM_BYTES, (cudaStream_t)stream>>>(
+      tq, tk, tv, (bf16*)out, ld_out, lse, cu, n_heads, n_heads / n_kv_heads, scale, pm);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <bool PREFIX>
+static int varlen_bwd(const char* who, const void* q, const void* k, const void* v, long long ld_qkv, const void* out,
+                      long long ld_out, const void* d_out, long long ld_dout, const float* lse, void* dq,
+                      long long ld_dq, void* dk, void* dv, long long ld_dkv, float* delta_ws, const int* cu, int nseq,
+                      int max_len, long long n_rows, int n_heads, int n_kv_heads, int head_dim, float scale,
+                      void* stream, const PrefixMap<PREFIX>& pm) {
+  int rc;
+  B200_REQUIRE(ld_dout % 8 == 0 && ((uintptr_t)d_out & 15) == 0, "%s: d_out must be 16-byte aligned", who);
+  B200_REQUIRE(dq != nullptr && ld_dq % 2 == 0 && ((uintptr_t)dq & 3) == 0 && ld_dkv % 2 == 0,
+               "%s: dq / dk / dv alignment", who);
+  const int g = n_heads / n_kv_heads;
+  CUtensorMap tq, tk, tv, tdo, tq2, tk2, tv2, tdo2;
+  if ((rc = make_packed_tmap(&tq, q, ld_qkv, n_rows, n_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_packed_tmap(&tdo, d_out, ld_dout, n_rows, n_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_packed_tmap(&tk, k, ld_qkv, n_rows, n_kv_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tv, v, ld_qkv, n_rows, n_kv_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tq2, q, ld_qkv, n_rows, n_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tdo2, d_out, ld_dout, n_rows, n_heads * head_dim, 128))) return rc;
+  if ((rc = make_packed_tmap(&tk2, k, ld_qkv, n_rows, n_kv_heads * head_dim, BWD_C))) return rc;
+  if ((rc = make_packed_tmap(&tv2, v, ld_qkv, n_rows, n_kv_heads * head_dim, BWD_C))) return rc;
+  auto dkv_kern = attention_varlen_bwd_dkv_kernel<PREFIX>;
+  auto dq_kern = attention_varlen_bwd_dq_kernel<PREFIX>;
+  B200_CHECK_CUDA(configure_smem_once((const void*)dkv_kern, (int)AttBwdCfg::SMEM_BYTES));
+  B200_CHECK_CUDA(configure_smem_once((const void*)dq_kern, (int)AttBwdCfg::SMEM_BYTES));
+  cudaStream_t st = (cudaStream_t)stream;
+  {
+    const long long total = n_rows * n_heads;
+    long long blocks = (total + 7) / 8;
+    if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
+    attention_varlen_delta_kernel<<<(int)blocks, 256, 0, st>>>((const bf16*)out, ld_out, (const bf16*)d_out, ld_dout,
+                                                               delta_ws, cu, nseq, n_rows, n_heads, head_dim);
+    B200_CHECK_CUDA(cudaGetLastError());
+  }
+  {
+    dim3 grid((max_len + 127) / 128, n_kv_heads, nseq);
+    dkv_kern<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(tq, tk, tv, tdo, lse, delta_ws, (bf16*)dk, (bf16*)dv,
+                                                               ld_dkv, cu, n_heads, g, scale, pm);
+    B200_CHECK_CUDA(cudaGetLastError());
+  }
+  {
+    dim3 grid((max_len + 127) / 128, n_heads, nseq);
+    dq_kern<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(tq2, tk2, tv2, tdo2, lse, delta_ws, (bf16*)dq, ld_dq, cu,
+                                                              n_heads, g, scale, pm);
+    B200_CHECK_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
 }  // namespace b200
 
 // Packed causal self-attention: q/k/v/out [n_rows][ld] bf16 (q, k, v may be column blocks of one fused qkv buffer);
@@ -1252,16 +1414,8 @@ extern "C" int rlaifv_attention_varlen_fwd(const void* q, const void* k, const v
   if ((rc = varlen_check("attention_varlen_fwd", ld_qkv, ld_out, out, nseq, max_len, n_rows, n_heads, n_kv_heads,
                          head_dim)))
     return rc;
-  CUtensorMap tq, tk, tv;
-  if ((rc = make_packed_tmap(&tq, q, ld_qkv, n_rows, n_heads * head_dim, ATT_BQ))) return rc;
-  if ((rc = make_packed_tmap(&tk, k, ld_qkv, n_rows, n_kv_heads * head_dim, ATT_BKV))) return rc;
-  if ((rc = make_packed_tmap(&tv, v, ld_qkv, n_rows, n_kv_heads * head_dim, ATT_BKV))) return rc;
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_varlen_fwd_kernel, (int)AttFwdCfg<128>::SMEM_BYTES));
-  dim3 grid((max_len + ATT_BQ - 1) / ATT_BQ, n_heads, nseq);
-  attention_varlen_fwd_kernel<<<grid, ATT_THREADS, AttFwdCfg<128>::SMEM_BYTES, (cudaStream_t)stream>>>(
-      tq, tk, tv, (bf16*)out, ld_out, lse, cu, n_heads, n_heads / n_kv_heads, scale);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return varlen_fwd<false>(q, k, v, ld_qkv, out, ld_out, lse, cu, nseq, max_len, n_rows, n_heads, n_kv_heads, head_dim,
+                           scale, stream, PrefixMap<false>{});
 }
 
 // Its backward: delta, the dK/dV kernel, then the dQ kernel, which writes bf16 dQ [n_rows][ld_dq] (may be the q column
@@ -1276,41 +1430,46 @@ extern "C" int rlaifv_attention_varlen_bwd(const void* q, const void* k, const v
   if ((rc = varlen_check("attention_varlen_bwd", ld_qkv, ld_out, (void*)out, nseq, max_len, n_rows, n_heads,
                          n_kv_heads, head_dim)))
     return rc;
-  B200_REQUIRE(ld_dout % 8 == 0 && ((uintptr_t)d_out & 15) == 0, "attention_varlen_bwd: d_out must be 16-byte aligned");
-  B200_REQUIRE(dq != nullptr && ld_dq % 2 == 0 && ((uintptr_t)dq & 3) == 0 && ld_dkv % 2 == 0,
-               "attention_varlen_bwd: dq / dk / dv alignment");
-  const int g = n_heads / n_kv_heads;
-  CUtensorMap tq, tk, tv, tdo, tq2, tk2, tv2, tdo2;
-  if ((rc = make_packed_tmap(&tq, q, ld_qkv, n_rows, n_heads * head_dim, BWD_C))) return rc;
-  if ((rc = make_packed_tmap(&tdo, d_out, ld_dout, n_rows, n_heads * head_dim, BWD_C))) return rc;
-  if ((rc = make_packed_tmap(&tk, k, ld_qkv, n_rows, n_kv_heads * head_dim, 128))) return rc;
-  if ((rc = make_packed_tmap(&tv, v, ld_qkv, n_rows, n_kv_heads * head_dim, 128))) return rc;
-  if ((rc = make_packed_tmap(&tq2, q, ld_qkv, n_rows, n_heads * head_dim, 128))) return rc;
-  if ((rc = make_packed_tmap(&tdo2, d_out, ld_dout, n_rows, n_heads * head_dim, 128))) return rc;
-  if ((rc = make_packed_tmap(&tk2, k, ld_qkv, n_rows, n_kv_heads * head_dim, BWD_C))) return rc;
-  if ((rc = make_packed_tmap(&tv2, v, ld_qkv, n_rows, n_kv_heads * head_dim, BWD_C))) return rc;
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_varlen_bwd_dkv_kernel, (int)AttBwdCfg::SMEM_BYTES));
-  B200_CHECK_CUDA(configure_smem_once((const void*)attention_varlen_bwd_dq_kernel, (int)AttBwdCfg::SMEM_BYTES));
-  cudaStream_t st = (cudaStream_t)stream;
-  {
-    const long long total = n_rows * n_heads;
-    long long blocks = (total + 7) / 8;
-    if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
-    attention_varlen_delta_kernel<<<(int)blocks, 256, 0, st>>>((const bf16*)out, ld_out, (const bf16*)d_out, ld_dout,
-                                                               delta_ws, cu, nseq, n_rows, n_heads, head_dim);
-    B200_CHECK_CUDA(cudaGetLastError());
-  }
-  {
-    dim3 grid((max_len + 127) / 128, n_kv_heads, nseq);
-    attention_varlen_bwd_dkv_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
-        tq, tk, tv, tdo, lse, delta_ws, (bf16*)dk, (bf16*)dv, ld_dkv, cu, n_heads, g, scale);
-    B200_CHECK_CUDA(cudaGetLastError());
-  }
-  {
-    dim3 grid((max_len + 127) / 128, n_heads, nseq);
-    attention_varlen_bwd_dq_kernel<<<grid, ATT_THREADS, AttBwdCfg::SMEM_BYTES, st>>>(
-        tq2, tk2, tv2, tdo2, lse, delta_ws, (bf16*)dq, ld_dq, cu, n_heads, g, scale);
-    B200_CHECK_CUDA(cudaGetLastError());
-  }
-  return 0;
+  return varlen_bwd<false>("attention_varlen_bwd", q, k, v, ld_qkv, out, ld_out, d_out, ld_dout, lse, dq, ld_dq, dk, dv,
+                           ld_dkv, delta_ws, cu, nseq, max_len, n_rows, n_heads, n_kv_heads, head_dim, scale, stream,
+                           PrefixMap<false>{});
+}
+
+// Packed causal self-attention with borrowed prefixes: the arguments of rlaifv_attention_varlen_fwd plus pos0 and
+// partner, int32 [nseq] host arrays (at most 64 sequences). Sequence s's own rows [cu[s], cu[s+1]) hold positions
+// pos0[s] .. pos0[s] + len_s - 1 (pos0 a multiple of 128); with pos0[s] > 0, positions t < pos0[s] are the rows
+// cu[partner[s]] + t of its lender, which holds at least pos0[s] rows and has partner = s and pos0 = 0. -1 = no partner.
+extern "C" int rlaifv_attention_varlen_prefix_fwd(const void* q, const void* k, const void* v, long long ld_qkv,
+                                                  void* out, long long ld_out, float* lse, const int* cu,
+                                                  const int* pos0, const int* partner, int nseq, int max_len,
+                                                  long long n_rows, int n_heads, int n_kv_heads, int head_dim,
+                                                  float scale, void* stream) {
+  int rc;
+  if ((rc = varlen_check("attention_varlen_prefix_fwd", ld_qkv, ld_out, out, nseq, max_len, n_rows, n_heads,
+                         n_kv_heads, head_dim)))
+    return rc;
+  PrefixMap<true> pm;
+  if ((rc = prefix_check("attention_varlen_prefix_fwd", pos0, partner, nseq, &pm))) return rc;
+  return varlen_fwd<true>(q, k, v, ld_qkv, out, ld_out, lse, cu, nseq, max_len, n_rows, n_heads, n_kv_heads, head_dim,
+                          scale, stream, pm);
+}
+
+// Its backward (arguments of rlaifv_attention_varlen_bwd plus pos0 / partner): dQ and dK/dV of own rows; a lender's
+// rows below its borrower's pos0 receive the sum of both sequences' dK/dV.
+extern "C" int rlaifv_attention_varlen_prefix_bwd(const void* q, const void* k, const void* v, long long ld_qkv,
+                                                  const void* out, long long ld_out, const void* d_out,
+                                                  long long ld_dout, const float* lse, void* dq, long long ld_dq,
+                                                  void* dk, void* dv, long long ld_dkv, float* delta_ws,
+                                                  const int* cu, const int* pos0, const int* partner, int nseq,
+                                                  int max_len, long long n_rows, int n_heads, int n_kv_heads,
+                                                  int head_dim, float scale, void* stream) {
+  int rc;
+  if ((rc = varlen_check("attention_varlen_prefix_bwd", ld_qkv, ld_out, (void*)out, nseq, max_len, n_rows, n_heads,
+                         n_kv_heads, head_dim)))
+    return rc;
+  PrefixMap<true> pm;
+  if ((rc = prefix_check("attention_varlen_prefix_bwd", pos0, partner, nseq, &pm))) return rc;
+  return varlen_bwd<true>("attention_varlen_prefix_bwd", q, k, v, ld_qkv, out, ld_out, d_out, ld_dout, lse, dq, ld_dq,
+                          dk, dv, ld_dkv, delta_ws, cu, nseq, max_len, n_rows, n_heads, n_kv_heads, head_dim, scale,
+                          stream, pm);
 }

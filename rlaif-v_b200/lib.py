@@ -103,6 +103,13 @@ _SIGNATURES = {
     "rlaifv_attention_varlen_bwd": [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p,
                                     c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_ll,
                                     c_int, c_int, c_int, c_float, c_void_p],
+    "rlaifv_attention_varlen_prefix_fwd": [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_int, c_int, c_ll, c_int, c_int, c_int, c_float,
+                                           c_void_p],
+    "rlaifv_attention_varlen_prefix_bwd": [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll,
+                                           c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_int, c_int, c_ll, c_int, c_int, c_int, c_float,
+                                           c_void_p],
     "rlaifv_rope_pos_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_void_p],
     "rlaifv_rope_pos_bwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_void_p],
     "rlaifv_dropout_rows_fwd": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, ctypes.c_ulonglong, c_void_p],

@@ -15,6 +15,7 @@ reduce-scatter / update / all-gather bucket slices in place.
 """
 import math
 from dataclasses import dataclass, field
+from typing import Optional
 
 import torch
 
@@ -262,20 +263,42 @@ class RowPacking:
     """Packed rows of a training forward (DESIGN.md §3). Sequence s keeps its first len_s rows, len_s = 1 + the last
     position whose spliced label is supervised (1 if there is none): attention is causal, so no supervised log-prob
     depends on a later row, and the compact head gives those rows exactly zero gradient. Sequence s occupies packed
-    rows [cu[s], cu[s] + len_s); packed row cu[s] + t is position t."""
+    rows [cu[s], cu[s] + len_s - pos0[s]); packed row cu[s] + t - pos0[s] is position t. With a shared prefix
+    (pos0[s] > 0, DESIGN.md §3 "Shared prompt prefixes") positions t < pos0[s] are the lender's rows
+    cu[partner[s]] + t; without one, pos0 is None and every sequence starts at position 0."""
     nseq: int
     T: int                   # padded length
-    M: int                   # packed rows: sum of len_s
-    max_len: int             # longest len_s
+    M: int                   # packed rows: sum of the own rows
+    max_len: int             # most own rows of a sequence
     cu: torch.Tensor         # int32 [nseq + 1]
     pos: torch.Tensor        # int32 [M]: position t of each packed row (its RoPE position)
     rows: torch.Tensor       # int32 [M]: the padded row s*T + t of each packed row
+    pos0: Optional[torch.Tensor] = None        # int32 [nseq] (device): first own position, a multiple of 128
+    partner: Optional[torch.Tensor] = None     # int32 [nseq] (device): lender of a borrower, borrower of a lender, or -1
+    pos0_h: Optional[torch.Tensor] = None      # the same two on the host (the attention entry points check them)
+    partner_h: Optional[torch.Tensor] = None
+
+    @property
+    def shared(self):
+        return self.pos0 is not None
 
     def packed_rows(self, row_pos):
-        """Padded rows s*T + t (-1 = unused slot, kept) -> packed rows cu[s] + t."""
+        """Padded rows s*T + t (-1 = unused slot, kept) -> packed rows (a borrower's t < pos0[s]: the lender's row)."""
         rp = row_pos.long().clamp(min=0)
         s = torch.div(rp, self.T, rounding_mode="floor")
-        return torch.where(row_pos >= 0, self.cu.long()[s] + rp - s * self.T, -1).to(torch.int32)
+        if self.pos0 is None:
+            return torch.where(row_pos >= 0, self.cu.long()[s] + rp - s * self.T, -1).to(torch.int32)
+        t = rp - s * self.T
+        p0 = self.pos0.long()[s]
+        cu = self.cu.long()
+        r = torch.where(t < p0, cu[self.partner.long()[s].clamp(min=0)] + t, cu[s] + t - p0)
+        return torch.where(row_pos >= 0, r, -1).to(torch.int32)
+
+
+# sequences one attention launch with shared prefixes takes (PREFIX_MAX_SEQ in csrc/attention.cu)
+PREFIX_MAX_SEQ = 64
+# shared prefixes end on a multiple of the attention kernels' 128-row tiles (why: DESIGN.md §3)
+PREFIX_ALIGN = 128
 
 
 def packed_lengths(labels):
@@ -284,20 +307,59 @@ def packed_lengths(labels):
     return (torch.where(labels != IGNORE_INDEX, t, -1).amax(dim=1) + 1).clamp(min=1)
 
 
-def pack_rows(labels):
-    """RowPacking of spliced labels [nseq, T], or None when every len_s is T. Reads the lengths to the host once."""
+def splice_sources(src, input_ids):
+    """What each spliced position holds, [nseq, T] int64: its token id, or the negative splice code of its image
+    feature row (or of padding). Two positions with equal values have equal decoder inputs."""
+    return torch.where(src >= 0, input_ids.gather(1, src.clamp(min=0).long()), src.long())
+
+
+def shared_prefix_lengths(labels, sources):
+    """pos0 of a preference batch [2b, T] (pair i = sequences i and b + i), int64 [2b] on the device: 0 for the
+    chosen side, and for the rejected side 128 * floor(min(p_i, f_i) / 128). p_i is the first position where the two
+    sides' sources differ (T if none); f_i the smaller of their first supervised rows (row t is supervised when the
+    label at t + 1 is; 0 for a side without one), so no shared row reaches the head."""
+    nseq, T = labels.shape
+    b = nseq // 2
+    t = torch.arange(T, device=labels.device)
+    p = torch.where(sources[:b] != sources[b:], t, T).amin(dim=1)
+    sup = labels[:, 1:] != IGNORE_INDEX
+    first = torch.where(sup.any(dim=1), torch.where(sup, t[:-1], T).amin(dim=1), 0)
+    f = torch.minimum(first[:b], first[b:])
+    pos0 = torch.div(torch.minimum(p, f), PREFIX_ALIGN, rounding_mode="floor") * PREFIX_ALIGN
+    return torch.cat([torch.zeros_like(pos0), pos0])
+
+
+def pack_rows(labels, sources=None):
+    """RowPacking of spliced labels [nseq, T], or None when it would drop no row. sources (splice_sources of a
+    preference batch, nseq = 2b): the rejected side of pair i also drops its first shared_prefix_lengths rows and
+    reads them from the chosen side. Reads the lengths to the host once."""
     nseq, T = labels.shape
     lens = packed_lengths(labels)
-    lens_h = lens.cpu()
-    M = int(lens_h.sum())
+    share = sources is not None and nseq % 2 == 0 and 0 < nseq <= PREFIX_MAX_SEQ
+    if share:
+        pos0 = shared_prefix_lengths(labels, sources)
+        lens_h, pos0_h = torch.stack([lens, pos0]).cpu()
+        share = bool(pos0_h.any())
+    else:
+        lens_h = lens.cpu()
+    own, own_h = (lens - pos0, lens_h - pos0_h) if share else (lens, lens_h)
+    M = int(own_h.sum())
     if M == nseq * T:
         return None
     dev = labels.device
     cu = torch.zeros(nseq + 1, dtype=torch.int64, device=dev)
-    cu[1:] = torch.cumsum(lens, 0)
-    seq = torch.repeat_interleave(torch.arange(nseq, device=dev), lens, output_size=M)
+    cu[1:] = torch.cumsum(own, 0)
+    seq = torch.repeat_interleave(torch.arange(nseq, device=dev), own, output_size=M)
     pos = torch.arange(M, device=dev) - cu[seq]
-    return RowPacking(nseq, T, M, int(lens_h.max()), cu.int(), pos.int(), (seq * T + pos).int())
+    if not share:
+        return RowPacking(nseq, T, M, int(own_h.max()), cu.int(), pos.int(), (seq * T + pos).int())
+    pos += pos0[seq]
+
+    def partners(p0):                        # built twice (device, host): an upload would wait for the stream
+        other = torch.arange(nseq, device=p0.device).roll(nseq // 2)
+        return torch.where((p0 > 0) | (p0.roll(nseq // 2) > 0), other, -1).int()
+    return RowPacking(nseq, T, M, int(own_h.max()), cu.int(), pos.int(), (seq * T + pos).int(),
+                      pos0.int(), partners(pos0), pos0_h.int(), partners(pos0_h))
 
 
 class ClipWeights:
@@ -393,6 +455,11 @@ class LlavaDPOPolicy:
         # the padded layout (the reference the packed path is tested against). A policy on the CPU only serves host-side
         # dry runs of the padded launch sequence, so it packs only when asked.
         self.pack_rows = self.device.type == "cuda"
+        # with packed rows: the rejected sequence of a pair reads the rows it shares with the chosen one (same inputs up
+        # to its first supervised row, whole 128-row tiles) from the chosen copy instead of computing them again
+        # (DESIGN.md §3 "Shared prompt prefixes"). Forward bits are unchanged; gradient sums change order. Not with
+        # LoRA dropout, which draws a separate mask for each copy.
+        self.share_prefix = False
         # SwiGLU backward inside the epilogue of the down-projection dgrad (no d(act) round trip, one launch less per
         # layer); False = separate swiglu_bwd pass
         self.fuse_swiglu_bwd = True
@@ -643,8 +710,8 @@ class LlavaDPOPolicy:
                                   lse=lse, n_kv_heads=nkv)
             else:
                 ops.rope_pos_fwd(qkv, cos, sin, pk.pos, nh, hd, n_kv_heads=nkv)
-                ops.attention_varlen_fwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], pk, nh, hd, scale, att, lse,
-                                         n_kv_heads=nkv)
+                att_fwd = ops.attention_varlen_prefix_fwd if pk.shared else ops.attention_varlen_fwd
+                att_fwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], pk, nh, hd, scale, att, lse, n_kv_heads=nkv)
             self._lin_fwd(i, "o", att, x2, residual=x, ls=ls if keep_stash else None)
             n2 = ops.rmsnorm_fwd(x2, P[f"l{i}.ln2"], d.rms_eps,
                                  out=torch.empty((M, H), dtype=_BF, device=dev) if extra else self.buf("n", (M, H)),
@@ -699,7 +766,10 @@ class LlavaDPOPolicy:
                                             T_hint=(T_hint, n_slots) if T_hint is not None else None)
         compact = keep_stash and self.compact_head
         # training on a ragged batch: the decoder runs only each sequence's rows up to its last supervised position
-        pk = pack_rows(new_labels) if compact and self.pack_rows else None
+        pk = None
+        if compact and self.pack_rows:
+            share = self.share_prefix and nseq == 2 * b and not (self.lora is not None and self.lora.dropout > 0.0)
+            pk = pack_rows(new_labels, splice_sources(src, input_ids) if share else None)
         if pk is not None:
             x = ops.rows_gather(pk.rows, x, out=self.buf("xp", (pk.M, H)))
         if keep_stash:
@@ -785,9 +855,10 @@ class LlavaDPOPolicy:
             qkv = ls["qkv"]
             dqkv = self.buf("dqkv", (M, H + 2 * KV))
             if pk is not None:
-                ops.attention_varlen_bwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], ls["att"], datt, ls["lse"], pk,
-                                         nh, hd, scale, dqkv[:, :H], dqkv[:, H:H + KV], dqkv[:, H + KV:],
-                                         self.buf("delta", (nh * M,), _F32), n_kv_heads=nkv)
+                att_bwd = ops.attention_varlen_prefix_bwd if pk.shared else ops.attention_varlen_bwd
+                att_bwd(qkv[:, :H], qkv[:, H:H + KV], qkv[:, H + KV:], ls["att"], datt, ls["lse"], pk, nh, hd, scale,
+                        dqkv[:, :H], dqkv[:, H:H + KV], dqkv[:, H + KV:], self.buf("delta", (nh * M,), _F32),
+                        n_kv_heads=nkv)
                 ops.rope_pos_bwd(dqkv, cos, sin, pk.pos, nh, hd, n_kv_heads=nkv)
             elif self.split_attention_bwd:
                 # dK/dV kernel + dQ kernel: dQ lands in the q block of dqkv as bf16, rotated back in place

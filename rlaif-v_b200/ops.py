@@ -137,6 +137,32 @@ def attention_varlen_bwd(q, k, v, out, d_out, lse, pk, n_heads, head_dim, scale,
     return dq, dk, dv
 
 
+def attention_varlen_prefix_fwd(q, k, v, pk, n_heads, head_dim, scale, out, lse, n_kv_heads=None):
+    """attention_varlen_fwd over a RowPacking whose borrowers read the rows below pk.pos0 from their lenders
+    (pk.pos0_h / pk.partner_h, DESIGN.md §3 "Shared prompt prefixes"); LSE holds own rows only."""
+    _chk(q), _chk(k), _chk(v), _chk(out), _chk(lse, _f32)
+    assert q.stride(0) == k.stride(0) == v.stride(0) and q.stride(1) == 1 and lse.numel() == n_heads * pk.M
+    _l.call("rlaifv_attention_varlen_prefix_fwd", _l.ptr(q), _l.ptr(k), _l.ptr(v), q.stride(0), _l.ptr(out),
+            out.stride(0), _l.ptr(lse), _l.ptr(pk.cu), _l.ptr(pk.pos0_h), _l.ptr(pk.partner_h), pk.nseq, pk.max_len,
+            pk.M, n_heads, n_heads if n_kv_heads is None else n_kv_heads, head_dim, float(scale), _l.stream_ptr())
+    return out, lse
+
+
+def attention_varlen_prefix_bwd(q, k, v, out, d_out, lse, pk, n_heads, head_dim, scale, dq, dk, dv, delta_ws,
+                                n_kv_heads=None):
+    """Backward of attention_varlen_prefix_fwd: a lender's rows below its borrower's pos0 receive both sequences'
+    dK/dV; everything else as attention_varlen_bwd."""
+    _chk(q), _chk(k), _chk(v), _chk(out), _chk(d_out), _chk(dq), _chk(dk), _chk(dv), _chk(lse, _f32)
+    _chk(delta_ws, _f32)
+    assert q.stride(0) == k.stride(0) == v.stride(0) and dk.stride(0) == dv.stride(0) and dq.stride(1) == 1
+    _l.call("rlaifv_attention_varlen_prefix_bwd", _l.ptr(q), _l.ptr(k), _l.ptr(v), q.stride(0), _l.ptr(out),
+            out.stride(0), _l.ptr(d_out), d_out.stride(0), _l.ptr(lse), _l.ptr(dq), dq.stride(0), _l.ptr(dk),
+            _l.ptr(dv), dk.stride(0), _l.ptr(delta_ws), _l.ptr(pk.cu), _l.ptr(pk.pos0_h), _l.ptr(pk.partner_h),
+            pk.nseq, pk.max_len, pk.M, n_heads, n_heads if n_kv_heads is None else n_kv_heads, head_dim, float(scale),
+            _l.stream_ptr())
+    return dq, dk, dv
+
+
 def cross_attention_fwd(q, k, v, nseq, Sq, Skv, n_heads, head_dim, scale, q_shared=True, out=None, lse=None):
     """Non-causal cross-attention: q [(1 if q_shared else nseq)*Sq, ld_q], k/v [nseq*Skv, ld_kv] (column blocks of
     one buffer allowed) -> out [nseq*Sq, n_heads*head_dim], lse [nseq, n_heads, Sq]."""

@@ -105,6 +105,8 @@ class TrainingArguments:                   # muffin/train/train_llava15.py:72-10
     seed: int = 42
     local_rank: int = -1
     micro_pairs: Optional[int] = None      # engine knob: pairs per micro-batch (None = whole batch)
+    # decoder rows a preference pair shares (prompt + image up to the first response token) computed once
+    share_prompt_prefix: bool = False
     # muffin/train/train_llava15_lora.py:112-117
     lora_enable: bool = False
     lora_r: int = 64
@@ -228,6 +230,7 @@ def init_model(model_args, data_args, training_args, attn_implementation=None, s
     state = load_hf_checkpoint(model_args.model_name_or_path, model_args.vision_tower)
     model = LlavaLlamaForCausalLM(dims, torch.device("cuda", local_rank), hf_state=state)
     model.config.use_cache = False
+    model.policy.share_prefix = bool(training_args.share_prompt_prefix)
     if training_args.lora_enable:
         if training_args.lora_bias != "none":
             raise NotImplementedError("lora_bias=%r (the shipped recipe uses 'none')" % training_args.lora_bias)
