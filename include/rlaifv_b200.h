@@ -7,8 +7,9 @@
  *    Nothing throws or aborts.
  *  - All pointers are raw DEVICE pointers owned by the caller (PyTorch storage in this repo);
  *    the library borrows them for the duration of the enqueued work and allocates nothing.
- *    One exception to the first rule: rlaifv_adamw_offload_bucket also takes pinned HOST pointers (the
- *    optimizer state the caller keeps in page-locked host memory); the caller owns those buffers too.
+ *    One exception to the first rule: rlaifv_adamw_offload_bucket and rlaifv_adamw8bit_offload_bucket also take
+ *    pinned HOST pointers (the optimizer state the caller keeps in page-locked host memory); the caller owns those
+ *    buffers too.
  *  - `stream` is a cudaStream_t (the caller's current stream); all work is enqueued asynchronously,
  *    no host synchronisation happens inside.
  *  - "bf16" = __nv_bfloat16 storage. Row-major everywhere; `ld*` = elements between rows.
@@ -17,6 +18,8 @@
  */
 #ifndef RLAIFV_B200_H_
 #define RLAIFV_B200_H_
+
+#include <stdint.h>
 
 #ifdef __cplusplus
 extern "C" {
@@ -332,10 +335,37 @@ int rlaifv_adamw_offload_bucket(float* host_master, float* host_exp_avg, float* 
                                 void* param_bf16, long long n, long long decay_n, float* ring, int n_slots,
                                 long long slot_elems, float lr, float beta1, float beta2, float eps, float weight_decay,
                                 int step, void* stream, void* h2d_stream, void* d2h_stream);
-/* Destroys the events rlaifv_adamw_offload_bucket keeps for `ring` on the current device (no-op if there are none).
- * Call it once the ring's work has completed and before the ring is freed; a later call with the same ring starts a
- * fresh set. */
-int rlaifv_adamw_offload_release(const float* ring);
+/* Destroys the events rlaifv_adamw_offload_bucket / rlaifv_adamw8bit_offload_bucket keep for `ring` on the current
+ * device (no-op if there are none). Call it once the ring's work has completed and before the ring is freed; a later
+ * call with the same ring starts a fresh set. */
+int rlaifv_adamw_offload_release(const void* ring);
+
+/* ---- AdamW with blockwise 8-bit moments (optim=adamw_bnb_8bit / adamw_8bit: bitsandbytes AdamW8bit, Dettmers et
+ * al. 2022, percentile clipping off). State per element: fp32 master, one uint8 code each for m and v; per block of
+ * 256 consecutive elements (counted from the slice's first element; the last block may be partial) one fp32
+ * absmax_m and absmax_v. m = map_m[code_m] * absmax_m, v = map_v[code_v] * absmax_v; map_m / map_v: the signed /
+ * unsigned 256-entry dynamic maps (device, strictly increasing fp32, zero2.dynamic_map). Per block: dequantize, the
+ * per-element arithmetic of rlaifv_adamw_step (grad_scale 1, weight decay on elements [0, decay_n)), write master and
+ * bf16(master), set absmax_m = max|m| and absmax_v = max v over the new fp32 moments, store for each element the code
+ * of the map entry nearest to m / absmax_m (v / absmax_v), ties to the lower index, the code of 0 for a zero absmax.
+ *
+ * One slice of n (% 8 == 0) elements on the device: codes n bytes each (8-byte aligned), absmax ceil(n / 256) floats
+ * each; master, grad and param_bf16 16-byte aligned. */
+int rlaifv_adamw8bit_step(float* master, uint8_t* code_m, uint8_t* code_v, float* absmax_m, float* absmax_v,
+                          const void* grad, void* param_bf16, long long n, long long decay_n, const float* map_m,
+                          const float* map_v, float lr, float beta1, float beta2, float eps, float weight_decay,
+                          int step, void* stream);
+/* The same update of one bucket whose state lives in PINNED HOST memory, through the chunk / slot / event pipeline of
+ * rlaifv_adamw_offload_bucket (same streams, same ordering, same release). host_master: n fp32; host_code_m /
+ * host_code_v: n bytes; host_absmax_m / host_absmax_v: ceil(n / 256) fp32. ring: caller-owned, 256-byte aligned device
+ * memory of n_slots (2..8) slots of slot_bytes = round_up(6 * slot_elems + 8 * slot_elems / 256, 256) bytes, each
+ * holding master | code_m | code_v | absmax_m | absmax_v of slot_elems (% 256 == 0) elements, so every chunk starts
+ * on a block edge. Bad sizes, misalignment and pageable host memory return -1. */
+int rlaifv_adamw8bit_offload_bucket(float* host_master, uint8_t* host_code_m, uint8_t* host_code_v,
+                                    float* host_absmax_m, float* host_absmax_v, const void* grad, void* param_bf16,
+                                    long long n, long long decay_n, const float* map_m, const float* map_v, void* ring,
+                                    int n_slots, long long slot_elems, float lr, float beta1, float beta2, float eps,
+                                    float weight_decay, int step, void* stream, void* h2d_stream, void* d2h_stream);
 
 #ifdef __cplusplus
 }

@@ -1202,6 +1202,111 @@ __global__ void adamw_staged_kernel(float* __restrict__ master, float* __restric
 }
 
 // ------------------------------------------------------------------------------------------------
+// AdamW with blockwise 8-bit moments (Dettmers et al., "8-bit Optimizers via Block-wise Quantization", 2022;
+// bitsandbytes AdamW8bit with percentile clipping off). State per element: the fp32 master and one uint8 code each for
+// m and v; per block of 256 consecutive elements one fp32 absmax each. m = map_m[code_m] * absmax_m and
+// v = map_v[code_v] * absmax_v, map_m / map_v being the signed / unsigned dynamic maps (256 strictly increasing fp32
+// values each, built by zero2.dynamic_map). A block's update: dequantize, adamw_elem, absmax_m = max|m| and
+// absmax_v = max v over the new fp32 moments, then store for each element the code of the map entry nearest to
+// m / absmax_m (v / absmax_v), ties to the lower index; a zero absmax stores the code of 0.
+// ------------------------------------------------------------------------------------------------
+static constexpr int kQBlock = 256;
+
+// Index of the entry of the sorted 256-entry map nearest to x, ties to the lower index: a binary search for the last
+// entry <= x (entry 0 if there is none), then one compare with its upper neighbour.
+__device__ __forceinline__ uint32_t quantize_nearest(const float* map, float x) {
+  int i = 0;
+#pragma unroll
+  for (int step = 128; step >= 1; step >>= 1)
+    if (map[i + step] <= x) i += step;
+  i = min(i, kQBlock - 2);
+  const float lo = map[i], hi = map[i + 1];
+  return (uint32_t)(i + (hi - x < x - lo ? 1 : 0));
+}
+
+// One block of the 8-bit update, run by one whole warp: lane l owns elements [8l, 8l + 8) of the block's first `cnt`
+// (a multiple of 8, at most 256). Pointers are at the block's first element (absmax_m / absmax_v at its entry);
+// elements below decay_n, counted from the block's first element, get weight decay. smap: map_m | map_v in shared
+// memory. adamw8bit_kernel runs it for the on-device and for the offloaded optimizer alike, so their results are
+// bit-identical.
+__device__ __forceinline__ void adamw8bit_block(float* __restrict__ master, uint8_t* __restrict__ qm,
+                                                uint8_t* __restrict__ qv, float* __restrict__ absmax_m,
+                                                float* __restrict__ absmax_v, const bf16* __restrict__ grad,
+                                                bf16* __restrict__ param_out, int cnt, long long decay_n,
+                                                const float* smap, float lr, float b1, float b2, float eps, float wd,
+                                                float bc1, float bc2_sqrt) {
+  const int lane = threadIdx.x & 31;
+  const int e0 = lane * 8;
+  const bool live = e0 < cnt;
+  float p[8], m[8], v[8];
+  float mx_m = 0.f, mx_v = 0.f;
+  if (live) {
+    const float4 p0 = reinterpret_cast<const float4*>(master + e0)[0];
+    const float4 p1 = reinterpret_cast<const float4*>(master + e0)[1];
+    const uint2 cm = *reinterpret_cast<const uint2*>(qm + e0);
+    const uint2 cv = *reinterpret_cast<const uint2*>(qv + e0);
+    float g[8];
+    load8(grad + e0, g);
+    const float am = *absmax_m, av = *absmax_v;
+    p[0] = p0.x; p[1] = p0.y; p[2] = p0.z; p[3] = p0.w; p[4] = p1.x; p[5] = p1.y; p[6] = p1.z; p[7] = p1.w;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t sh = 8 * (j & 3);
+      m[j] = smap[((j < 4 ? cm.x : cm.y) >> sh) & 255] * am;
+      v[j] = smap[kQBlock + (((j < 4 ? cv.x : cv.y) >> sh) & 255)] * av;
+      adamw_elem(p[j], m[j], v[j], g[j], lr, b1, b2, eps, e0 + j < decay_n ? wd : 0.f, bc1, bc2_sqrt, 1.f);
+      mx_m = fmaxf(mx_m, fabsf(m[j]));
+      mx_v = fmaxf(mx_v, v[j]);
+    }
+    reinterpret_cast<float4*>(master + e0)[0] = make_float4(p[0], p[1], p[2], p[3]);
+    reinterpret_cast<float4*>(master + e0)[1] = make_float4(p[4], p[5], p[6], p[7]);
+    store8(param_out + e0, p);
+  }
+  mx_m = warp_max(mx_m);
+  mx_v = warp_max(mx_v);
+  if (live) {
+    uint2 om = make_uint2(0u, 0u), ov = make_uint2(0u, 0u);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t sh = 8 * (j & 3);
+      const uint32_t c_m = quantize_nearest(smap, mx_m > 0.f ? m[j] / mx_m : 0.f);
+      const uint32_t c_v = quantize_nearest(smap + kQBlock, mx_v > 0.f ? v[j] / mx_v : 0.f);
+      (j < 4 ? om.x : om.y) |= c_m << sh;
+      (j < 4 ? ov.x : ov.y) |= c_v << sh;
+    }
+    *reinterpret_cast<uint2*>(qm + e0) = om;
+    *reinterpret_cast<uint2*>(qv + e0) = ov;
+  }
+  if (lane == 0) {
+    *absmax_m = mx_m;
+    *absmax_v = mx_v;
+  }
+}
+
+// The 8-bit update of n elements (n % 8 == 0) whose blocks start at element 0: one warp per 256-element block, the
+// last block partial when n % 256 != 0. The on-device optimizer launches it on a slice, the offloaded one on a chunk
+// staged in a ring slot.
+__global__ void __launch_bounds__(256) adamw8bit_kernel(float* __restrict__ master, uint8_t* __restrict__ qm,
+                                                        uint8_t* __restrict__ qv, float* __restrict__ absmax_m,
+                                                        float* __restrict__ absmax_v, const bf16* __restrict__ grad,
+                                                        bf16* __restrict__ param_out, long long n, long long decay_n,
+                                                        const float* __restrict__ map_m,
+                                                        const float* __restrict__ map_v, float lr, float b1, float b2,
+                                                        float eps, float wd, float bc1, float bc2_sqrt) {
+  __shared__ float smap[2 * kQBlock];
+  for (int i = threadIdx.x; i < 2 * kQBlock; i += blockDim.x) smap[i] = i < kQBlock ? map_m[i] : map_v[i - kQBlock];
+  __syncthreads();
+  const long long nblk = (n + kQBlock - 1) / kQBlock;
+  const int warps = blockDim.x >> 5;
+  for (long long b = (long long)blockIdx.x * warps + (threadIdx.x >> 5); b < nblk; b += (long long)gridDim.x * warps) {
+    const long long e = b * kQBlock;
+    const int cnt = n - e < kQBlock ? (int)(n - e) : kQBlock;
+    adamw8bit_block(master + e, qm + e, qv + e, absmax_m + b, absmax_v + b, grad + e, param_out + e, cnt,
+                    decay_n - e, smap, lr, b1, b2, eps, wd, bc1, bc2_sqrt);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Dropout for the LoRA adapter input (peft lora.Linear: lora_B(lora_A(dropout(x))), p = 0.05 in
 // muffin/train/train_llava15_lora.py:115). Stateless counter-based RNG: the keep bit of element i
 // is a hash of (seed, i), so the backward regenerates the mask instead of storing it.
@@ -1643,7 +1748,7 @@ struct OffloadEvents {
   bool ready = false;
 };
 static std::mutex g_offload_mu;
-static std::map<std::pair<int, const float*>, OffloadEvents> g_offload_pool;
+static std::map<std::pair<int, const void*>, OffloadEvents> g_offload_pool;
 
 static void destroy_offload_events(OffloadEvents& e) {
   for (int s = 0; s < kOffloadMaxSlots; ++s)
@@ -1655,7 +1760,7 @@ static void destroy_offload_events(OffloadEvents& e) {
   e.ready = false;
 }
 
-static int offload_events(const float* ring, OffloadEvents** out) {
+static int offload_events(const void* ring, OffloadEvents** out) {
   int dev = 0;
   B200_CHECK_CUDA(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lock(g_offload_mu);
@@ -1697,6 +1802,34 @@ static int require_memory_type(const void* p, size_t bytes, cudaMemoryType want,
   return 0;
 }
 
+// The chunk / slot / event rotation of both offloaded optimizers. [0, n) is cut into chunks of slot_elems (the last one
+// shorter); chunk i takes the next slot s of the ring's rotation: load(s, off, c, h2d) enqueues its H2D copies on h2d
+// after the slot's previous store, update(s, off, c) its kernel on cs once they are done, store(s, off, c, d2h) its D2H
+// copies on d2h once that is done. The streams run up to n_slots chunks apart, so with 3 slots the load of chunk i+1,
+// the update of chunk i and the store of chunk i-1 overlap. Each callback returns 0 or the entry point's error code.
+template <class Load, class Update, class Store>
+static int offload_pipeline(const void* ring, int n_slots, long long n, long long slot_elems, cudaStream_t hs,
+                            cudaStream_t cs, cudaStream_t ds, Load load, Update update, Store store) {
+  OffloadEvents* ev = nullptr;
+  int rc;
+  if ((rc = offload_events(ring, &ev)) != 0) return rc;
+  for (long long off = 0; off < n; off += slot_elems) {
+    const long long c = n - off < slot_elems ? n - off : slot_elems;
+    const int s = ev->next_slot % n_slots;
+    ev->next_slot = (s + 1) % n_slots;
+    B200_CHECK_CUDA(cudaStreamWaitEvent(hs, ev->stored[s], 0));
+    if ((rc = load(s, off, c, hs)) != 0) return rc;
+    B200_CHECK_CUDA(cudaEventRecord(ev->loaded[s], hs));
+    B200_CHECK_CUDA(cudaStreamWaitEvent(cs, ev->loaded[s], 0));
+    if ((rc = update(s, off, c)) != 0) return rc;
+    B200_CHECK_CUDA(cudaEventRecord(ev->updated[s], cs));
+    B200_CHECK_CUDA(cudaStreamWaitEvent(ds, ev->updated[s], 0));
+    if ((rc = store(s, off, c, ds)) != 0) return rc;
+    B200_CHECK_CUDA(cudaEventRecord(ev->stored[s], ds));
+  }
+  return 0;
+}
+
 extern "C" int rlaifv_adamw_offload_bucket(float* host_master, float* host_exp_avg, float* host_exp_avg_sq,
                                            const void* grad, void* param_bf16, long long n, long long decay_n,
                                            float* ring, int n_slots, long long slot_elems, float lr, float beta1,
@@ -1720,46 +1853,152 @@ extern "C" int rlaifv_adamw_offload_bucket(float* host_master, float* host_exp_a
   if ((rc = require_memory_type(ring, (size_t)n_slots * 3 * slot_elems * sizeof(float), cudaMemoryTypeDevice,
                                 "ring")) != 0)
     return rc;
-  OffloadEvents* ev = nullptr;
-  if ((rc = offload_events(ring, &ev)) != 0) return rc;
-
   const float bc1 = 1.f - powf(beta1, (float)step);
   const float bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
-  cudaStream_t cs = (cudaStream_t)stream, hs = (cudaStream_t)h2d_stream, ds = (cudaStream_t)d2h_stream;
+  cudaStream_t cs = (cudaStream_t)stream;
   const bf16* g = (const bf16*)grad;
   bf16* p = (bf16*)param_bf16;
-  // chunk i: H2D on hs (after the slot's previous store), update on cs, D2H on ds. The streams run up to n_slots
-  // chunks apart, so with 3 slots the load of chunk i+1, the update of chunk i and the store of chunk i-1 overlap.
-  for (long long off = 0; off < n; off += slot_elems) {
-    const long long c = n - off < slot_elems ? n - off : slot_elems;
+  auto slot = [&](int s) { return ring + (size_t)s * 3 * slot_elems; };     // master | m | v
+  auto load = [&](int s, long long off, long long c, cudaStream_t hs) -> int {
     const size_t cb = (size_t)c * sizeof(float);
-    const int s = ev->next_slot % n_slots;
-    ev->next_slot = (s + 1) % n_slots;
-    float* sm = ring + (size_t)s * 3 * slot_elems;
-    float* smm = sm + slot_elems;
-    float* sv = smm + slot_elems;
-    B200_CHECK_CUDA(cudaStreamWaitEvent(hs, ev->stored[s], 0));
-    B200_CHECK_CUDA(cudaMemcpyAsync(sm, host_master + off, cb, cudaMemcpyHostToDevice, hs));
-    B200_CHECK_CUDA(cudaMemcpyAsync(smm, host_exp_avg + off, cb, cudaMemcpyHostToDevice, hs));
-    B200_CHECK_CUDA(cudaMemcpyAsync(sv, host_exp_avg_sq + off, cb, cudaMemcpyHostToDevice, hs));
-    B200_CHECK_CUDA(cudaEventRecord(ev->loaded[s], hs));
-    B200_CHECK_CUDA(cudaStreamWaitEvent(cs, ev->loaded[s], 0));
+    B200_CHECK_CUDA(cudaMemcpyAsync(slot(s), host_master + off, cb, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(slot(s) + slot_elems, host_exp_avg + off, cb, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(slot(s) + 2 * slot_elems, host_exp_avg_sq + off, cb, cudaMemcpyHostToDevice, hs));
+    return 0;
+  };
+  auto update = [&](int s, long long off, long long c) -> int {
     long long dn = decay_n - off;
     dn = dn < 0 ? 0 : (dn > c ? c : dn);
-    adamw_staged_kernel<<<grid_for(c / 4, 256, 16), 256, 0, cs>>>(sm, smm, sv, g + off, p + off, c, dn, lr, beta1,
-                                                                   beta2, eps, weight_decay, bc1, bc2_sqrt);
+    adamw_staged_kernel<<<grid_for(c / 4, 256, 16), 256, 0, cs>>>(slot(s), slot(s) + slot_elems,
+                                                                   slot(s) + 2 * slot_elems, g + off, p + off, c, dn,
+                                                                   lr, beta1, beta2, eps, weight_decay, bc1, bc2_sqrt);
     B200_CHECK_CUDA(cudaGetLastError());
-    B200_CHECK_CUDA(cudaEventRecord(ev->updated[s], cs));
-    B200_CHECK_CUDA(cudaStreamWaitEvent(ds, ev->updated[s], 0));
-    B200_CHECK_CUDA(cudaMemcpyAsync(host_master + off, sm, cb, cudaMemcpyDeviceToHost, ds));
-    B200_CHECK_CUDA(cudaMemcpyAsync(host_exp_avg + off, smm, cb, cudaMemcpyDeviceToHost, ds));
-    B200_CHECK_CUDA(cudaMemcpyAsync(host_exp_avg_sq + off, sv, cb, cudaMemcpyDeviceToHost, ds));
-    B200_CHECK_CUDA(cudaEventRecord(ev->stored[s], ds));
-  }
+    return 0;
+  };
+  auto store = [&](int s, long long off, long long c, cudaStream_t ds) -> int {
+    const size_t cb = (size_t)c * sizeof(float);
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_master + off, slot(s), cb, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_exp_avg + off, slot(s) + slot_elems, cb, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_exp_avg_sq + off, slot(s) + 2 * slot_elems, cb, cudaMemcpyDeviceToHost, ds));
+    return 0;
+  };
+  return offload_pipeline(ring, n_slots, n, slot_elems, (cudaStream_t)h2d_stream, cs, (cudaStream_t)d2h_stream, load,
+                          update, store);
+}
+
+// Byte size of one ring slot of the 8-bit offloaded optimizer for slot_elems (% 256 == 0) elements: master (fp32) |
+// code_m | code_v (uint8) | absmax_m | absmax_v (fp32, one per 256 elements), rounded up to 256 bytes so that every
+// slot starts 256-byte aligned. zero2.adamw8bit_slot_bytes sizes the ring by the same formula.
+static inline size_t adamw8bit_slot_bytes(long long slot_elems) {
+  const size_t raw = (size_t)slot_elems * 6 + (size_t)(slot_elems / kQBlock) * 2 * sizeof(float);
+  return (raw + 255) / 256 * 256;
+}
+
+extern "C" int rlaifv_adamw8bit_step(float* master, uint8_t* code_m, uint8_t* code_v, float* absmax_m,
+                                     float* absmax_v, const void* grad, void* param_bf16, long long n,
+                                     long long decay_n, const float* map_m, const float* map_v, float lr, float beta1,
+                                     float beta2, float eps, float weight_decay, int step, void* stream) {
+  B200_REQUIRE(n > 0 && n % 8 == 0 && step >= 1, "adamw8bit: n <= 0, n %% 8 != 0 or step < 1");
+  B200_REQUIRE(decay_n >= 0 && decay_n <= n, "adamw8bit: decay_n %lld outside [0, %lld]", decay_n, n);
+  B200_REQUIRE(((uintptr_t)master & 15) == 0 && ((uintptr_t)grad & 15) == 0 && ((uintptr_t)param_bf16 & 15) == 0 &&
+                   ((uintptr_t)code_m & 7) == 0 && ((uintptr_t)code_v & 7) == 0 && ((uintptr_t)absmax_m & 3) == 0 &&
+                   ((uintptr_t)absmax_v & 3) == 0,
+               "adamw8bit: master / grad / param not 16-byte, codes not 8-byte or absmax not 4-byte aligned");
+  B200_REQUIRE(map_m != nullptr && map_v != nullptr, "adamw8bit: map_m / map_v is NULL");
+  const float bc1 = 1.f - powf(beta1, (float)step);
+  const float bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
+  adamw8bit_kernel<<<grid_for((n + kQBlock - 1) / kQBlock, 8, 8), 256, 0, ST>>>(
+      master, code_m, code_v, absmax_m, absmax_v, (const bf16*)grad, (bf16*)param_bf16, n, decay_n, map_m, map_v, lr,
+      beta1, beta2, eps, weight_decay, bc1, bc2_sqrt);
+  B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
-extern "C" int rlaifv_adamw_offload_release(const float* ring) {
+extern "C" int rlaifv_adamw8bit_offload_bucket(float* host_master, uint8_t* host_code_m, uint8_t* host_code_v,
+                                               float* host_absmax_m, float* host_absmax_v, const void* grad,
+                                               void* param_bf16, long long n, long long decay_n, const float* map_m,
+                                               const float* map_v, void* ring, int n_slots, long long slot_elems,
+                                               float lr, float beta1, float beta2, float eps, float weight_decay,
+                                               int step, void* stream, void* h2d_stream, void* d2h_stream) {
+  B200_REQUIRE(n > 0 && n % 8 == 0 && step >= 1, "adamw8bit_offload: n <= 0, n %% 8 != 0 or step < 1");
+  B200_REQUIRE(decay_n >= 0 && decay_n <= n, "adamw8bit_offload: decay_n %lld outside [0, %lld]", decay_n, n);
+  B200_REQUIRE(n_slots >= 2 && n_slots <= kOffloadMaxSlots, "adamw8bit_offload: n_slots %d outside [2, %d]", n_slots,
+               kOffloadMaxSlots);
+  B200_REQUIRE(slot_elems > 0 && slot_elems % kQBlock == 0,
+               "adamw8bit_offload: slot_elems %lld not a positive multiple of 256", slot_elems);
+  B200_REQUIRE(((uintptr_t)grad & 15) == 0 && ((uintptr_t)param_bf16 & 15) == 0 && ((uintptr_t)ring & 255) == 0,
+               "adamw8bit_offload: grad / param not 16-byte or ring not 256-byte aligned");
+  const long long nblk = (n + kQBlock - 1) / kQBlock;
+  const size_t slot_bytes = adamw8bit_slot_bytes(slot_elems);
+  int rc;
+  if ((rc = require_memory_type(host_master, (size_t)n * 4, cudaMemoryTypeHost, "host_master")) != 0) return rc;
+  if ((rc = require_memory_type(host_code_m, (size_t)n, cudaMemoryTypeHost, "host_code_m")) != 0) return rc;
+  if ((rc = require_memory_type(host_code_v, (size_t)n, cudaMemoryTypeHost, "host_code_v")) != 0) return rc;
+  if ((rc = require_memory_type(host_absmax_m, (size_t)nblk * 4, cudaMemoryTypeHost, "host_absmax_m")) != 0) return rc;
+  if ((rc = require_memory_type(host_absmax_v, (size_t)nblk * 4, cudaMemoryTypeHost, "host_absmax_v")) != 0) return rc;
+  if ((rc = require_memory_type(grad, (size_t)n * 2, cudaMemoryTypeDevice, "grad")) != 0) return rc;
+  if ((rc = require_memory_type(param_bf16, (size_t)n * 2, cudaMemoryTypeDevice, "param_bf16")) != 0) return rc;
+  if ((rc = require_memory_type(map_m, kQBlock * 4, cudaMemoryTypeDevice, "map_m")) != 0) return rc;
+  if ((rc = require_memory_type(map_v, kQBlock * 4, cudaMemoryTypeDevice, "map_v")) != 0) return rc;
+  if ((rc = require_memory_type(ring, (size_t)n_slots * slot_bytes, cudaMemoryTypeDevice, "ring")) != 0) return rc;
+
+  const float bc1 = 1.f - powf(beta1, (float)step);
+  const float bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
+  cudaStream_t cs = (cudaStream_t)stream;
+  const bf16* g = (const bf16*)grad;
+  bf16* p = (bf16*)param_bf16;
+  // slot s: master | code_m | code_v | absmax_m | absmax_v (adamw8bit_slot_bytes). Chunks start at multiples of
+  // slot_elems, so on block edges, and chunk blocks are the bucket's blocks [off / 256, off / 256 + ceil(c / 256)).
+  struct Slot {
+    float* master;
+    uint8_t *qm, *qv;
+    float *am, *av;
+  };
+  auto slot = [&](int s) {
+    uint8_t* base = (uint8_t*)ring + (size_t)s * slot_bytes;
+    Slot t;
+    t.master = (float*)base;
+    t.qm = base + (size_t)slot_elems * 4;
+    t.qv = t.qm + slot_elems;
+    t.am = (float*)(t.qv + slot_elems);
+    t.av = t.am + slot_elems / kQBlock;
+    return t;
+  };
+  auto load = [&](int s, long long off, long long c, cudaStream_t hs) -> int {
+    const Slot t = slot(s);
+    const long long b0 = off / kQBlock, nb = (c + kQBlock - 1) / kQBlock;
+    B200_CHECK_CUDA(cudaMemcpyAsync(t.master, host_master + off, (size_t)c * 4, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(t.qm, host_code_m + off, (size_t)c, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(t.qv, host_code_v + off, (size_t)c, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(t.am, host_absmax_m + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, hs));
+    B200_CHECK_CUDA(cudaMemcpyAsync(t.av, host_absmax_v + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, hs));
+    return 0;
+  };
+  auto update = [&](int s, long long off, long long c) -> int {
+    const Slot t = slot(s);
+    long long dn = decay_n - off;
+    dn = dn < 0 ? 0 : (dn > c ? c : dn);
+    adamw8bit_kernel<<<grid_for((c + kQBlock - 1) / kQBlock, 8, 8), 256, 0, cs>>>(
+        t.master, t.qm, t.qv, t.am, t.av, g + off, p + off, c, dn, map_m, map_v, lr, beta1, beta2, eps, weight_decay,
+        bc1, bc2_sqrt);
+    B200_CHECK_CUDA(cudaGetLastError());
+    return 0;
+  };
+  auto store = [&](int s, long long off, long long c, cudaStream_t ds) -> int {
+    const Slot t = slot(s);
+    const long long b0 = off / kQBlock, nb = (c + kQBlock - 1) / kQBlock;
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_master + off, t.master, (size_t)c * 4, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_code_m + off, t.qm, (size_t)c, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_code_v + off, t.qv, (size_t)c, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_absmax_m + b0, t.am, (size_t)nb * 4, cudaMemcpyDeviceToHost, ds));
+    B200_CHECK_CUDA(cudaMemcpyAsync(host_absmax_v + b0, t.av, (size_t)nb * 4, cudaMemcpyDeviceToHost, ds));
+    return 0;
+  };
+  return offload_pipeline(ring, n_slots, n, slot_elems, (cudaStream_t)h2d_stream, cs, (cudaStream_t)d2h_stream, load,
+                          update, store);
+}
+
+extern "C" int rlaifv_adamw_offload_release(const void* ring) {
   int dev = 0;
   B200_CHECK_CUDA(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lock(g_offload_mu);

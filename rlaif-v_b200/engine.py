@@ -27,7 +27,10 @@ class DPOStepEngine:
     def __init__(self, policy: LlavaDPOPolicy, lr=5e-7, weight_decay=0.01, betas=(0.9, 0.999), eps=1e-8,
                  total_steps=2672, warmup_ratio=0.05, dpo_use_average=False, micro_pairs=None,
                  rank=0, world=1, group=None, constant_lr=False, hf_deepspeed_input_cast=False,
-                 dpo_token_weighted=False, offload_optimizer=False, offload_budget=None, batch_pairs=None):
+                 dpo_token_weighted=False, offload_optimizer=False, offload_budget=None, batch_pairs=None,
+                 optim="adamw_torch"):
+        """optim: the optimizer state format, "adamw_torch" (fp32 moments) or "adamw_8bit" (blockwise 8-bit moments,
+        zero2.state_format of --optim adamw_bnb_8bit / adamw_8bit)."""
         self.policy = policy
         self.rank, self.world, self.group = rank, world, group
         if offload_optimizer:
@@ -48,10 +51,11 @@ class DPOStepEngine:
                 reserve = policy.activation_reserve_bytes(pairs, d.max_len)
             self.opt = OffloadAdamW(policy.trainable_buckets(), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
                                     rank=rank, world=world, group=group, gather_order=policy.param_need_order(),
-                                    device_budget=offload_budget, activation_reserve=reserve)
+                                    device_budget=offload_budget, activation_reserve=reserve, optim=optim)
         else:
             self.opt = Zero2AdamW(policy.trainable_buckets(), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
-                                  rank=rank, world=world, group=group, gather_order=policy.param_need_order())
+                                  rank=rank, world=world, group=group, gather_order=policy.param_need_order(),
+                                  optim=optim)
         self.base_lr, self.total_steps, self.warmup_ratio = lr, total_steps, warmup_ratio
         self.constant_lr = constant_lr
         self.dpo_use_average = dpo_use_average

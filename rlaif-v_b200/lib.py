@@ -75,6 +75,11 @@ _SIGNATURES = {
     "rlaifv_adamw_offload_bucket": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_int, c_ll,
                                     c_float, c_float, c_float, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p],
     "rlaifv_adamw_offload_release": [c_void_p],
+    "rlaifv_adamw8bit_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_void_p,
+                              c_void_p, c_float, c_float, c_float, c_float, c_float, c_int, c_void_p],
+    "rlaifv_adamw8bit_offload_bucket": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_ll,
+                                        c_void_p, c_void_p, c_void_p, c_int, c_ll, c_float, c_float, c_float, c_float,
+                                        c_float, c_int, c_void_p, c_void_p, c_void_p],
     "rlaifv_attention_fwd_gqa": [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_int, c_int,
                                  c_int, c_int, c_int, c_int, c_float, c_void_p],
     "rlaifv_attention_bwd_gqa": [c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p,

@@ -571,6 +571,42 @@ def adamw_offload_release(ring):
     _l.call("rlaifv_adamw_offload_release", _l.ptr(ring))
 
 
+def adamw8bit_step(master, code_m, code_v, absmax_m, absmax_v, grad, param_bf16, decay_n, map_m, map_v, lr, beta1,
+                   beta2, eps, weight_decay, step):
+    """AdamW with blockwise 8-bit moments on one slice of n elements (blocks of 256 from its first element): fp32
+    master, uint8 codes [n], fp32 absmax [ceil(n / 256)], bf16 grad / param [n]. Elements [0, decay_n) get weight
+    decay. map_m / map_v: the signed / unsigned dynamic maps on the device (zero2.dynamic_map)."""
+    _chk(master, _f32), _chk(code_m, torch.uint8), _chk(code_v, torch.uint8), _chk(absmax_m, _f32)
+    _chk(absmax_v, _f32), _chk(grad), _chk(param_bf16), _chk(map_m, _f32), _chk(map_v, _f32)
+    n = master.numel()
+    nb = (n + 255) // 256
+    assert code_m.numel() == n and code_v.numel() == n and grad.numel() == n and param_bf16.numel() == n
+    assert absmax_m.numel() == nb and absmax_v.numel() == nb and map_m.numel() == 256 and map_v.numel() == 256
+    _l.call("rlaifv_adamw8bit_step", _l.ptr(master), _l.ptr(code_m), _l.ptr(code_v), _l.ptr(absmax_m),
+            _l.ptr(absmax_v), _l.ptr(grad), _l.ptr(param_bf16), n, int(decay_n), _l.ptr(map_m), _l.ptr(map_v),
+            float(lr), float(beta1), float(beta2), float(eps), float(weight_decay), int(step), _l.stream_ptr())
+
+
+def adamw8bit_offload_bucket(host_master, host_code_m, host_code_v, host_absmax_m, host_absmax_v, grad, param_bf16,
+                             decay_n, map_m, map_v, ring, slot_elems, lr, beta1, beta2, eps, weight_decay, step,
+                             h2d_stream, d2h_stream):
+    """adamw8bit_step of one bucket whose state is in pinned host memory, streamed through the device staging `ring`
+    ([n_slots, zero2.adamw8bit_slot_bytes(slot_elems)] uint8) on h2d_stream -> the current launch stream ->
+    d2h_stream. Pinned-ness is checked by the library (a pageable tensor raises B200Error)."""
+    n = host_master.numel()
+    nb = (n + 255) // 256
+    for t, dt, k in ((host_master, _f32, n), (host_code_m, torch.uint8, n), (host_code_v, torch.uint8, n),
+                     (host_absmax_m, _f32, nb), (host_absmax_v, _f32, nb)):
+        assert t.dtype == dt and t.device.type == "cpu" and t.is_contiguous() and t.numel() == k
+    _chk(ring, torch.uint8), _chk(param_bf16), _chk(grad), _chk(map_m, _f32), _chk(map_v, _f32)
+    assert grad.numel() == n and param_bf16.numel() == n and ring.dim() == 2
+    _l.call("rlaifv_adamw8bit_offload_bucket", _l.ptr(host_master), _l.ptr(host_code_m), _l.ptr(host_code_v),
+            _l.ptr(host_absmax_m), _l.ptr(host_absmax_v), _l.ptr(grad), _l.ptr(param_bf16), n, int(decay_n),
+            _l.ptr(map_m), _l.ptr(map_v), _l.ptr(ring), ring.shape[0], int(slot_elems), float(lr), float(beta1),
+            float(beta2), float(eps), float(weight_decay), int(step), _l.stream_ptr(),
+            _l.c_void_p(h2d_stream.cuda_stream), _l.c_void_p(d2h_stream.cuda_stream))
+
+
 def gemm_dual(a, b, a2, b2, out, *, k2, r, n_sub=0, b_mn=False, residual=None, accumulate=False):
     """out (+)= a @ op(b)^T + a2[:, koff:koff+k2] @ op(b2)^T (+ residual), one fp32 accumulator.
     koff = (n0 // n_sub) * r per output tile when n_sub > 0, else 0."""

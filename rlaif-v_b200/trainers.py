@@ -26,7 +26,7 @@ import torch.distributed as dist
 
 from . import ops
 from .engine import DPOStepEngine, METRIC_NAMES
-from .zero2 import OffloadAdamW
+from .zero2 import OffloadAdamW, state_format
 
 _F32 = torch.float32
 
@@ -212,6 +212,7 @@ class LLaVA15DPOTrainer:
                                     micro_pairs=getattr(a, "micro_pairs", None), rank=self.rank, world=self.world,
                                     offload_optimizer=bool(getattr(a, "offload_optimizer", False)),
                                     batch_pairs=getattr(a, "per_device_train_batch_size", None),
+                                    optim=state_format(getattr(a, "optim", "adamw_torch")),
                                     hf_deepspeed_input_cast=bool(getattr(a, "bf16", True) and getattr(a, "deepspeed", None)),
                                     constant_lr=getattr(a, "lr_scheduler_type", "cosine") == "constant")
         self.state = {"global_step": 0, "log_history": []}

@@ -4,8 +4,8 @@ script/train/llava15_train.sh:31-34).
 
 Every bucket of ParamStore (embed | layer i | head | projector) is cut into `world` equal slices;
 rank r owns slice r of every bucket: fp32 master weights and Adam moments exist only for owned
-slices (12 B/param / world), gradients are reduce-scattered in place into the owned slice as soon
-as a bucket's backward has finished (overlapping the rest of the backward on a side stream), the
+slices (12 B/param / world; about 6 B with optim="adamw_8bit"), gradients are reduce-scattered in
+place into the owned slice as soon as a bucket's backward has finished (overlapping the rest of the backward on a side stream), the
 fused AdamW kernel updates the slice and writes bf16 straight into the parameter buffer, and an
 in-place all-gather redistributes the updated parameters.  With world == 1 the collectives vanish.
 OffloadAdamW (world == 1) keeps the state that does not fit on the device in pinned host memory and
@@ -23,6 +23,67 @@ from . import lib as _lib
 from . import ops
 
 _F32 = torch.float32
+_U8 = torch.uint8
+
+# ---- optimizer state formats ------------------------------------------------------------------------------------------
+# adamw_torch: fp32 master, exp_avg and exp_avg_sq (12 B per element; torch.optim.AdamW, the default).
+# adamw_8bit: fp32 master, one uint8 code each for exp_avg and exp_avg_sq, and per block of QBLOCK consecutive elements
+# of a slice one fp32 absmax each (bitsandbytes AdamW8bit, Dettmers et al. 2022; HF --optim adamw_bnb_8bit / adamw_8bit).
+# Blocks are counted from the start of each owned slice; a slice's last block may be partial.
+OPTIMS = ("adamw_torch", "adamw_8bit")
+QBLOCK = 256
+STATE_BYTES_PER_ELEM = 12            # adamw_torch: fp32 master + exp_avg + exp_avg_sq
+
+
+def state_format(hf_optim):
+    """The state format of an HF TrainingArguments.optim value: adamw_bnb_8bit and adamw_8bit (HF's alias) train with
+    8-bit moments; every other value keeps the fp32 AdamW state."""
+    return "adamw_8bit" if hf_optim in ("adamw_bnb_8bit", "adamw_8bit") else "adamw_torch"
+
+
+def _check_optim(optim):
+    if optim not in OPTIMS:
+        raise ValueError("optimizer state format %r: expected one of %s" % (optim, ", ".join(OPTIMS)))
+
+
+def n_blocks(n):
+    """Quantization blocks of a slice of n elements."""
+    return (n + QBLOCK - 1) // QBLOCK
+
+
+def state_bytes(n, optim="adamw_torch"):
+    """Exact bytes of optimizer state of one slice of n elements."""
+    _check_optim(optim)
+    return STATE_BYTES_PER_ELEM * n if optim == "adamw_torch" else 6 * n + 8 * n_blocks(n)
+
+
+def state_parts(optim):
+    """The flat state tensors of a format, as (name, dtype, "elem" | "block"): one entry per element of the owned slices,
+    or one per quantization block. The names are the state_dict keys and the optimizer's attribute names."""
+    _check_optim(optim)
+    if optim == "adamw_torch":
+        return (("master", _F32, "elem"), ("exp_avg", _F32, "elem"), ("exp_avg_sq", _F32, "elem"))
+    return (("master", _F32, "elem"), ("exp_avg_q", _U8, "elem"), ("exp_avg_sq_q", _U8, "elem"),
+            ("absmax", _F32, "block"), ("absmax_sq", _F32, "block"))
+
+
+def dynamic_map(signed):
+    """The 256-entry code map of 8-bit AdamW, built as bitsandbytes' create_dynamic_map builds it: for i in 0..6, the
+    midpoints of linspace(0.1, 1, k) with k = 2^i + 1 (signed) or 2^(i+1) + 1 (unsigned), scaled by 10^(i-6), and for
+    the signed map their negatives too; then 0 and 1. Strictly increasing fp32."""
+    vals = [torch.tensor([0.0, 1.0], dtype=_F32)]
+    for i in range(7):
+        k = 2 ** i + 1 if signed else 2 ** (i + 1) + 1
+        b = torch.linspace(0.1, 1, k, dtype=_F32)
+        pos = 10 ** (i - 6) * ((b[:-1] + b[1:]) / 2)
+        vals += [pos, -pos] if signed else [pos]
+    return torch.sort(torch.cat(vals)).values
+
+
+def _initial_code(name):
+    """What a fresh state tensor holds: the code of 0 for the moments (index 127 of the signed map, 0 of the unsigned
+    one), zero for the rest (master is copied from the parameters)."""
+    return 127 if name == "exp_avg_q" else 0
 
 
 def cosine_lr(step, total_steps, base_lr, warmup_ratio=0.05):
@@ -45,7 +106,10 @@ class OptBucket:
 
 class Zero2AdamW:
     def __init__(self, buckets, lr=5e-7, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, rank=0, world=1,
-                 group=None, gather_order=None):
+                 group=None, gather_order=None, optim="adamw_torch"):
+        """optim: the state format, "adamw_torch" (fp32 moments) or "adamw_8bit" (blockwise 8-bit moments)."""
+        _check_optim(optim)
+        self.optim = optim
         self.buckets = list(buckets)
         self.index = {b.name: i for i, b in enumerate(self.buckets)}
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
@@ -53,13 +117,20 @@ class Zero2AdamW:
         self.step_count = 0
         dev = self.buckets[0].flat.device
         self.slices = []   # (bucket, s0, s1, offset into the owned fp32 state), s0/s1 relative to the bucket
-        total = 0
+        self.block_offsets = []     # per slice: its first block in the owned block-indexed state (absmax, absmax_sq)
+        total = blocks = 0
         for b in self.buckets:
             assert b.size % (world * 8) == 0, (b.name, b.size)
             n = b.size // world
             self.slices.append((b, rank * n, (rank + 1) * n, total))
+            self.block_offsets.append(blocks)
             total += n
-        self.owned = total
+            blocks += n_blocks(n)
+        self.owned, self.owned_blocks = total, blocks
+        self.state_nbytes = sum(state_bytes(s1 - s0, optim) for _, s0, s1, _ in self.slices)
+        if optim == "adamw_8bit":
+            self.map_m = dynamic_map(True).to(dev)
+            self.map_v = dynamic_map(False).to(dev)
         self._init_state(dev)
         self.comm_stream = torch.cuda.Stream(device=dev) if world > 1 else None
         self.opt_stream = None
@@ -70,11 +141,18 @@ class Zero2AdamW:
         self.gather_order = [self.index[n] for n in gather_order if n in self.index] if gather_order else \
             list(range(len(self.buckets)))
 
+    def _new_state(self, n_elems, n_blk, device, prefix=""):
+        """Fresh flat state tensors of this format (state_parts) for n_elems elements in n_blk blocks, set as the
+        attributes prefix + name. The master is left for the caller to fill."""
+        for name, dtype, per in state_parts(self.optim):
+            shape = (n_elems if per == "elem" else n_blk,)
+            t = torch.empty(shape, dtype=dtype, device=device) if name == "master" else \
+                torch.full(shape, _initial_code(name), dtype=dtype, device=device)
+            setattr(self, prefix + name, t)
+
     def _init_state(self, dev):
-        """fp32 master copy of the owned slices and zeroed moments, all on the device."""
-        self.master = torch.empty(self.owned, dtype=_F32, device=dev)
-        self.exp_avg = torch.zeros(self.owned, dtype=_F32, device=dev)
-        self.exp_avg_sq = torch.zeros(self.owned, dtype=_F32, device=dev)
+        """fp32 master copy of the owned slices and fresh moments, all on the device."""
+        self._new_state(self.owned, self.owned_blocks, dev)
         for b, s0, s1, o in self.slices:
             self.master[o:o + (s1 - s0)].copy_(b.flat[s0:s1])
 
@@ -104,6 +182,14 @@ class Zero2AdamW:
     def _adamw_bucket(self, bi, lr):
         b, s0, s1, o = self.slices[bi]
         b1, b2 = self.betas
+        if self.optim == "adamw_8bit":      # one launch per slice: blocks never split at the decay edge
+            n, q = s1 - s0, self.block_offsets[bi]
+            nb = n_blocks(n)
+            ops.adamw8bit_step(self.master[o:o + n], self.exp_avg_q[o:o + n], self.exp_avg_sq_q[o:o + n],
+                               self.absmax[q:q + nb], self.absmax_sq[q:q + nb], b.grad[s0:s1], b.flat[s0:s1],
+                               min(n, max(0, b.decay_size - s0)), self.map_m, self.map_v, lr, b1, b2, self.eps,
+                               self.wd, self.step_count)
+            return
         dec_end = min(s1, b.decay_size)
         if dec_end > s0:
             n = dec_end - s0
@@ -179,9 +265,23 @@ class Zero2AdamW:
         for bi in list(self._gathered):
             self.wait_bucket(bi)
 
+    def _format_keys(self):
+        """state_dict entries that record the format: none for adamw_torch (its checkpoints predate the choice)."""
+        return {} if self.optim == "adamw_torch" else {"optim": self.optim, "block": QBLOCK}
+
     def state_dict(self):
-        return {"step": self.step_count, "master": self.master, "exp_avg": self.exp_avg,
-                "exp_avg_sq": self.exp_avg_sq, "rank": self.rank, "world": self.world}
+        return {"step": self.step_count, **{k: getattr(self, k) for k, _, _ in state_parts(self.optim)},
+                **self._format_keys(), "rank": self.rank, "world": self.world}
+
+    def check_format(self, sd):
+        """Refuse (ValueError) a checkpoint written with the other optimizer state format."""
+        fmt = sd.get("optim", "adamw_torch")
+        if sd.get("block", QBLOCK) != QBLOCK:
+            fmt = "%s (blocks of %s)" % (fmt, sd["block"])
+        if fmt != self.optim:
+            raise ValueError("optimizer checkpoint holds %s state, but this optimizer keeps %s state: converting "
+                             "between formats is not supported; resume with the --optim it was written with"
+                             % (fmt, self.optim))
 
     def check_state_size(self, sd):
         """Refuse (ValueError) a checkpoint whose flat state was written for another set of trainable buckets."""
@@ -193,11 +293,11 @@ class Zero2AdamW:
 
     def load_state_dict(self, sd):
         assert sd["world"] == self.world and sd["rank"] == self.rank
+        self.check_format(sd)
         self.check_state_size(sd)
         self.step_count = sd["step"]
-        self.master.copy_(sd["master"])
-        self.exp_avg.copy_(sd["exp_avg"])
-        self.exp_avg_sq.copy_(sd["exp_avg_sq"])
+        for k, _, _ in state_parts(self.optim):
+            getattr(self, k).copy_(sd[k])
 
 
 # ------------------------------------------------------------------------------------------------
@@ -205,8 +305,7 @@ class Zero2AdamW:
 # through a small device staging ring each step (DeepSpeed `offload_optimizer: {device: cpu}`, script/zero2_offload.json;
 # the update itself stays on the GPU). DESIGN.md §2 has the memory plan, §3 the pipeline.
 # ------------------------------------------------------------------------------------------------
-STATE_BYTES_PER_ELEM = 12            # fp32 master + exp_avg + exp_avg_sq
-DEFAULT_SLOT_ELEMS = 8 << 20         # 8 Mi elements: 96 MB per ring slot (master | m | v)
+DEFAULT_SLOT_ELEMS = 8 << 20         # 8 Mi elements: 96 MB per ring slot (master | m | v), 48 MB with 8-bit moments
 DEFAULT_SLOTS = 3                    # load of chunk i+1 | update of chunk i | store of chunk i-1
 DEVICE_MARGIN = 2 << 30              # allocator fragmentation, CLIP tower and head buffers, library workspaces
 HOST_MARGIN = 8 << 30                # what MemAvailable must still show after the streamed state is pinned
@@ -231,17 +330,35 @@ def offload_priority(names):
     return rest + eva_embed + eva + layers + head
 
 
-def offload_plan(sizes, budget_bytes, bytes_per_elem=STATE_BYTES_PER_ELEM):
+def offload_plan(sizes, budget_bytes, optim="adamw_torch"):
     """Resident / streamed split of the optimizer state. sizes: [(bucket name, elements)]. Buckets are taken in
-    offload_priority order while their state fits in budget_bytes; the first one that does not fit and every one after
-    it are streamed. Returns (resident names, streamed names), each in priority order."""
+    offload_priority order while their state (state_bytes in format `optim`) fits in budget_bytes; the first one that
+    does not fit and every one after it are streamed. Returns (resident names, streamed names), each in priority order."""
     n_of = dict(sizes)
     order = offload_priority([n for n, _ in sizes])
     used, k = 0, 0
-    while k < len(order) and used + n_of[order[k]] * bytes_per_elem <= budget_bytes:
-        used += n_of[order[k]] * bytes_per_elem
+    while k < len(order) and used + state_bytes(n_of[order[k]], optim) <= budget_bytes:
+        used += state_bytes(n_of[order[k]], optim)
         k += 1
     return order[:k], order[k:]
+
+
+def ring_slot_elems(largest, slot_elems, optim="adamw_torch"):
+    """Elements per staging-ring slot: slot_elems, or less when the largest owned slice is smaller (rounded up to 4
+    elements for adamw_torch, to a whole block for adamw_8bit, whose chunks must start on block edges)."""
+    q = 4 if optim == "adamw_torch" else QBLOCK
+    return min(slot_elems, (largest + q - 1) // q * q)
+
+
+def adamw8bit_slot_bytes(slot_elems):
+    """Bytes of one 8-bit ring slot: master | code_m | code_v | absmax_m | absmax_v of slot_elems (% 256 == 0) elements,
+    rounded up to 256 bytes (the layout rlaifv_adamw8bit_offload_bucket reads)."""
+    return (6 * slot_elems + 8 * (slot_elems // QBLOCK) + 255) // 256 * 256
+
+
+def ring_bytes(n_slots, slot_elems, optim="adamw_torch"):
+    """Device bytes of the staging ring."""
+    return n_slots * (3 * slot_elems * 4 if optim == "adamw_torch" else adamw8bit_slot_bytes(slot_elems))
 
 
 def offload_chunks(n, slot_elems, decay_size):
@@ -340,7 +457,7 @@ def _read_meminfo(path="/proc/meminfo"):
 
 
 class OffloadAdamW(Zero2AdamW):
-    """Zero2AdamW for one GPU whose fp32 state does not all fit on the device. offload_plan keeps as many buckets'
+    """Zero2AdamW for one GPU whose optimizer state does not all fit on the device. offload_plan keeps as many buckets'
     state on the device as `device_budget` allows (resident buckets run the on-device path unchanged); the others'
     state is in pinned host memory and rlaifv_adamw_offload_bucket streams it through a staging ring of n_slots x
     slot_elems on two copy streams while the update runs on the optimizer stream. Results are bit-identical to
@@ -355,64 +472,72 @@ class OffloadAdamW(Zero2AdamW):
 
     def __init__(self, buckets, lr=5e-7, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, rank=0, world=1,
                  group=None, gather_order=None, device_budget=None, activation_reserve=0,
-                 slot_elems=DEFAULT_SLOT_ELEMS, n_slots=DEFAULT_SLOTS, host_margin=HOST_MARGIN, meminfo=None):
+                 slot_elems=DEFAULT_SLOT_ELEMS, n_slots=DEFAULT_SLOTS, host_margin=HOST_MARGIN, meminfo=None,
+                 optim="adamw_torch"):
         if world != 1:
             raise NotImplementedError("offload_optimizer runs on one GPU; with two or more, ZeRO-2 shards the state "
                                       "(offloading each rank's slice is not implemented)")
-        assert slot_elems > 0 and slot_elems % 4 == 0 and 2 <= n_slots <= 8
+        assert slot_elems > 0 and slot_elems % (4 if optim == "adamw_torch" else QBLOCK) == 0 and 2 <= n_slots <= 8
         self._cfg = dict(device_budget=device_budget, activation_reserve=activation_reserve, slot_elems=slot_elems,
                          n_slots=n_slots, host_margin=host_margin, meminfo=meminfo)
         self._host = []
         self._stored = {}
         self.ring = None
         super().__init__(buckets, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, rank=rank, world=world,
-                         group=group, gather_order=gather_order)
+                         group=group, gather_order=gather_order, optim=optim)
 
     def _init_state(self, dev):
         cfg = self._cfg
         largest = max(s1 - s0 for _, s0, s1, _ in self.slices)
-        self.slot_elems = min(cfg["slot_elems"], (largest + 3) // 4 * 4)
-        ring_bytes = cfg["n_slots"] * 3 * self.slot_elems * 4
+        self.slot_elems = ring_slot_elems(largest, cfg["slot_elems"], self.optim)
+        ring_b = ring_bytes(cfg["n_slots"], self.slot_elems, self.optim)
         budget = cfg["device_budget"]
         if budget is None:
-            budget = torch.cuda.mem_get_info(dev)[0] - cfg["activation_reserve"] - ring_bytes - DEVICE_MARGIN
+            budget = torch.cuda.mem_get_info(dev)[0] - cfg["activation_reserve"] - ring_b - DEVICE_MARGIN
         self.device_budget = budget
         self.resident_names, self.streamed_names = offload_plan(
-            [(b.name, s1 - s0) for b, s0, s1, _ in self.slices], budget)
+            [(b.name, s1 - s0) for b, s0, s1, _ in self.slices], budget, self.optim)
         streamed = set(self.streamed_names)
         self._global = [o for _, _, _, o in self.slices]       # offsets in the checkpoint's flat layout
+        self._global_blocks = list(self.block_offsets)         # block offsets in the checkpoint's flat layout
         self._is_streamed = [b.name in streamed for b, _, _, _ in self.slices]
-        local, n_dev, n_host = [], 0, 0
+        local, local_blocks, n_dev, n_host, nb_dev, nb_host = [], [], 0, 0, 0, 0
+        host_bytes = 0
         for (b, s0, s1, _), st in zip(self.slices, self._is_streamed):
             local.append(n_host if st else n_dev)
+            local_blocks.append(nb_host if st else nb_dev)
             if st:
                 n_host += s1 - s0
+                nb_host += n_blocks(s1 - s0)
+                host_bytes += state_bytes(s1 - s0, self.optim)
             else:
                 n_dev += s1 - s0
+                nb_dev += n_blocks(s1 - s0)
         self.resident_elems, self.streamed_elems = n_dev, n_host
         if n_host:
-            check_host_memory(STATE_BYTES_PER_ELEM * n_host, (cfg["meminfo"] or _read_meminfo)(), cfg["host_margin"])
+            check_host_memory(host_bytes, (cfg["meminfo"] or _read_meminfo)(), cfg["host_margin"])
         # resident buckets index the device tensors exactly as Zero2AdamW does (so _adamw_bucket is reused as is);
         # streamed buckets index the host tensors
         self.slices = [(b, s0, s1, lo) for (b, s0, s1, _), lo in zip(self.slices, local)]
-        self.master = torch.empty(n_dev, dtype=_F32, device=dev)
-        self.exp_avg = torch.zeros(n_dev, dtype=_F32, device=dev)
-        self.exp_avg_sq = torch.zeros(n_dev, dtype=_F32, device=dev)
+        self.block_offsets = local_blocks
+        self._new_state(n_dev, nb_dev, dev)
         # Plain CPU tensors of the exact size, pinned with cudaHostRegister: torch's pinned allocator rounds every block
         # up to a power of two, which would turn ~45 GB of state into 64 GB.
-        self.host_master = torch.empty(n_host, dtype=_F32)
-        self.host_exp_avg = torch.zeros(n_host, dtype=_F32)
-        self.host_exp_avg_sq = torch.zeros(n_host, dtype=_F32)
-        for t in (self.host_master, self.host_exp_avg, self.host_exp_avg_sq):
+        self._new_state(n_host, nb_host, "cpu", prefix="host_")
+        for name, _, _ in state_parts(self.optim):
+            t = getattr(self, "host_" + name)
             if t.numel():
                 self._register(t)
         for (b, s0, s1, o), st in zip(self.slices, self._is_streamed):
             (self.host_master if st else self.master)[o:o + (s1 - s0)].copy_(b.flat[s0:s1])
         if n_host:
-            self.ring = torch.empty((cfg["n_slots"], 3 * self.slot_elems), dtype=_F32, device=dev)
+            if self.optim == "adamw_torch":
+                self.ring = torch.empty((cfg["n_slots"], 3 * self.slot_elems), dtype=_F32, device=dev)
+            else:
+                self.ring = torch.empty((cfg["n_slots"], adamw8bit_slot_bytes(self.slot_elems)), dtype=_U8, device=dev)
             self.h2d_stream = torch.cuda.Stream(device=dev)
             self.d2h_stream = torch.cuda.Stream(device=dev)
-        self.pinned_bytes = sum(t.numel() * 4 for t in self._host)
+        self.pinned_bytes = sum(t.numel() * t.element_size() for t in self._host)
 
     def _register(self, t):
         rt = torch.cuda.cudart()
@@ -459,49 +584,65 @@ class OffloadAdamW(Zero2AdamW):
         if prev is not None:                 # this step's loads read what the last step's stores wrote
             self.h2d_stream.wait_event(prev)
         b1, b2 = self.betas
-        ops.adamw_offload_bucket(self.host_master[o:o + n], self.host_exp_avg[o:o + n], self.host_exp_avg_sq[o:o + n],
-                                 b.grad[s0:s1], b.flat[s0:s1], min(n, max(0, b.decay_size - s0)), self.ring,
-                                 self.slot_elems, lr, b1, b2, self.eps, self.wd, self.step_count, self.h2d_stream,
-                                 self.d2h_stream)
+        decay_n = min(n, max(0, b.decay_size - s0))
+        if self.optim == "adamw_8bit":
+            q, nb = self.block_offsets[bi], n_blocks(n)
+            ops.adamw8bit_offload_bucket(self.host_master[o:o + n], self.host_exp_avg_q[o:o + n],
+                                         self.host_exp_avg_sq_q[o:o + n], self.host_absmax[q:q + nb],
+                                         self.host_absmax_sq[q:q + nb], b.grad[s0:s1], b.flat[s0:s1], decay_n,
+                                         self.map_m, self.map_v, self.ring, self.slot_elems, lr, b1, b2, self.eps,
+                                         self.wd, self.step_count, self.h2d_stream, self.d2h_stream)
+        else:
+            ops.adamw_offload_bucket(self.host_master[o:o + n], self.host_exp_avg[o:o + n],
+                                     self.host_exp_avg_sq[o:o + n], b.grad[s0:s1], b.flat[s0:s1], decay_n, self.ring,
+                                     self.slot_elems, lr, b1, b2, self.eps, self.wd, self.step_count, self.h2d_stream,
+                                     self.d2h_stream)
         ev = torch.cuda.Event()
         ev.record(self.d2h_stream)
         self._stored[bi] = ev
 
     def _state_parts(self):
-        return (("master", self.master, self.host_master), ("exp_avg", self.exp_avg, self.host_exp_avg),
-                ("exp_avg_sq", self.exp_avg_sq, self.host_exp_avg_sq))
+        """(name, device tensor, host tensor, checkpoint length, [(global offset, local offset, length)] per slice) of
+        every state tensor."""
+        out = []
+        for name, _, per in state_parts(self.optim):
+            spans = []
+            for (b, s0, s1, o), g, q, gq in zip(self.slices, self._global, self.block_offsets, self._global_blocks):
+                spans.append((g, o, s1 - s0) if per == "elem" else (gq, q, n_blocks(s1 - s0)))
+            total = self.owned if per == "elem" else self.owned_blocks
+            out.append((name, getattr(self, name), getattr(self, "host_" + name), total, spans))
+        return out
 
     def state_dict(self):
-        """The Zero2AdamW layout (full flat fp32 tensors, here on the host), so either optimizer resumes the other's
-        checkpoint. The three tensors take 12 B per parameter of host memory on top of the pinned state (81 GB at 7B):
-        MemAvailable is checked first, so a checkpoint that does not fit raises MemoryError instead of waking the
-        kernel's OOM killer."""
-        check_host_memory(STATE_BYTES_PER_ELEM * self.owned, (self._cfg["meminfo"] or _read_meminfo)(),
-                          self._cfg["host_margin"])
+        """The Zero2AdamW layout (full flat tensors, here on the host), so either optimizer resumes the other's
+        checkpoint of the same format. The tensors take state_bytes per slice of host memory on top of the pinned state
+        (81 GB at 7B with fp32 moments): MemAvailable is checked first, so a checkpoint that does not fit raises
+        MemoryError instead of waking the kernel's OOM killer."""
+        check_host_memory(self.state_nbytes, (self._cfg["meminfo"] or _read_meminfo)(), self._cfg["host_margin"])
         self.wait_all()
         torch.cuda.current_stream().synchronize()
         if self.opt_stream is not None:
             self.opt_stream.synchronize()
         self._drain()
         out = {}
-        for key, dev_t, host_t in self._state_parts():
-            full = torch.empty(self.owned, dtype=_F32)
-            for (b, s0, s1, o), g, st in zip(self.slices, self._global, self._is_streamed):
-                full[g:g + (s1 - s0)].copy_((host_t if st else dev_t)[o:o + (s1 - s0)])
+        for key, dev_t, host_t, total, spans in self._state_parts():
+            full = torch.empty(total, dtype=dev_t.dtype)
+            for (g, o, n), st in zip(spans, self._is_streamed):
+                full[g:g + n].copy_((host_t if st else dev_t)[o:o + n])
             out[key] = full
-        return {"step": self.step_count, "master": out["master"], "exp_avg": out["exp_avg"],
-                "exp_avg_sq": out["exp_avg_sq"], "rank": self.rank, "world": self.world}
+        return {"step": self.step_count, **out, **self._format_keys(), "rank": self.rank, "world": self.world}
 
     def load_state_dict(self, sd):
         assert sd["world"] == self.world and sd["rank"] == self.rank
+        self.check_format(sd)
         self.check_state_size(sd)
         self.wait_all()
         if self.opt_stream is not None:
             self.opt_stream.synchronize()
         self._drain()
         self.step_count = sd["step"]
-        for key, dev_t, host_t in self._state_parts():
+        for key, dev_t, host_t, _, spans in self._state_parts():
             src = sd[key]
-            for (b, s0, s1, o), g, st in zip(self.slices, self._global, self._is_streamed):
-                (host_t if st else dev_t)[o:o + (s1 - s0)].copy_(src[g:g + (s1 - s0)])
+            for (g, o, n), st in zip(spans, self._is_streamed):
+                (host_t if st else dev_t)[o:o + n].copy_(src[g:g + n])
         torch.cuda.current_stream().synchronize()

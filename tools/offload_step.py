@@ -18,6 +18,19 @@
 
     python tools/offload_step.py --omnilmm --tune-clip {0,1} --out DIR [--max-len 1024] [--micro-pairs 2]
 
+    python tools/offload_step.py --optim adamw_8bit --out DIR [--steps 5] [--warmup 3]
+
+AdamW with blockwise 8-bit moments, written to DIR/offload_step_8bit.json (each leg can be skipped, see --help):
+1. Kernel throughput: rlaifv_adamw8bit_step against the fp32 adamw_kernel on one 2^30-element shard, CUDA events, GB/s
+   of algorithmic bytes (master 8 B, grad / param 4 B, codes 2 B per element, absmax 16 B per 256).
+2. Identity: LLaVA-1.5-7B widths at --identity-layers layers, three steps on the device, then offloaded with a mixed
+   and an all-streamed split: metrics, bf16 parameters, master, codes and absmax bit for bit.
+3. Loss trajectory: 7B widths at 2 layers, 20 steps of each optimizer from one seed on bench.py's inputs: the largest
+   |delta loss| and the master weights' relative difference.
+4. Config (b) offloaded with adamw_torch and adamw_8bit, alternating (torch, 8-bit, torch, 8-bit) in one process.
+5. 13B full fine-tuning (1 pair at 2048 tokens per micro-batch) and OmniLMM-12B with a trained tower, with 8-bit
+   moments: measured where MemAvailable holds the streamed state, otherwise the refusal with MemAvailable recorded.
+
 OmniLMM-12B (config d), written to DIR/offload_step_omnilmm.json:
 1. Identity at OmniLMM widths, --identity-layers decoder layers and --identity-eva-blocks EVA blocks, in both tower
    modes: three steps on the device, then three from the same seed offloaded with a mixed split (embed, resampler and
@@ -66,6 +79,12 @@ def parse_args(argv=None):
     ap.add_argument("--identity-eva-blocks", type=int, default=4)
     ap.add_argument("--skip-config-d", action="store_true")
     ap.add_argument("--skip-trained-tower", action="store_true")
+    ap.add_argument("--optim", choices=("adamw_torch", "adamw_8bit"), default="adamw_torch",
+                    help="adamw_8bit: the 8-bit legs (kernel, identity, loss trajectory, config (b) both ways, 13B, "
+                         "trained-tower OmniLMM) instead of the legs above")
+    ap.add_argument("--skip-kernel", action="store_true")
+    ap.add_argument("--skip-trajectory", action="store_true")
+    ap.add_argument("--skip-13b", action="store_true")
     args = ap.parse_args(argv)
     if args.max_len is None:
         args.max_len = 1024 if args.omnilmm else 2048
@@ -82,12 +101,12 @@ def gpu_name_and_power():
         return "unknown (%s)" % e, None
 
 
-def make_engine(layers, micro, offload_budget=None, offload=False, seed=0):
+def make_engine(layers, micro, offload_budget=None, offload=False, seed=0, optim="adamw_torch"):
     from rlaifv_b200.engine import DPOStepEngine
     from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
     policy = LlavaDPOPolicy(LlavaDims(num_layers=layers), torch.device("cuda", 0), seed=seed)
     eng = DPOStepEngine(policy, lr=5e-7, weight_decay=0.01, total_steps=2672, micro_pairs=micro,
-                        offload_optimizer=offload, offload_budget=offload_budget)
+                        offload_optimizer=offload, offload_budget=offload_budget, optim=optim)
     return eng
 
 
@@ -211,7 +230,7 @@ def ring_alone_gbs(opt, reps=3):
             "gbs_each_way": reps * 12 * n / (ms * 1e-3) / 1e9}
 
 
-def config_b(args):
+def config_b(args, optim="adamw_torch"):
     """Config (b) through the engine's own default device budget, as `train_llava15.py --deepspeed
     script/zero2_offload.json --micro_pairs M --model_max_length L` plans it."""
     from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
@@ -221,10 +240,10 @@ def config_b(args):
     gc.collect()
     torch.cuda.empty_cache()
     policy = LlavaDPOPolicy(dims, torch.device("cuda", 0), seed=0)
-    return timed_offload_run(args, policy, [bench.synthetic_batch(0, s, B) for s in range(2)], B, T)
+    return timed_offload_run(args, policy, [bench.synthetic_batch(0, s, B) for s in range(2)], B, T, optim)
 
 
-def timed_offload_run(args, policy, host_batches, B, T):
+def timed_offload_run(args, policy, host_batches, B, T, optim="adamw_torch"):
     """The measured run of a full-size policy with the engine's own default device budget for --micro-pairs at
     dims.max_len: step 0 against ln 2, --warmup and --steps timed steps, then the copy rates."""
     from rlaifv_b200.engine import DPOStepEngine
@@ -235,7 +254,7 @@ def timed_offload_run(args, policy, host_batches, B, T):
     reserve = policy.activation_reserve_bytes(micro, dims.max_len)
     t0 = time.perf_counter()
     eng = DPOStepEngine(policy, lr=5e-7, weight_decay=0.01, total_steps=2672, micro_pairs=micro,
-                        offload_optimizer=True, batch_pairs=B)
+                        offload_optimizer=True, batch_pairs=B, optim=optim)
     setup_s = time.perf_counter() - t0
     opt = eng.opt
     add_reference_logps(policy, host_batches, B, micro)
@@ -291,7 +310,8 @@ def timed_offload_run(args, policy, host_batches, B, T):
 
     # copy rates the streams achieved: one more step with each offloaded bucket's H2D / D2H spans event-timed
     spans = []
-    orig_off = z.ops.adamw_offload_bucket
+    entry = "adamw_offload_bucket" if optim == "adamw_torch" else "adamw8bit_offload_bucket"
+    orig_off = getattr(z.ops, entry)
 
     def timed_off(hm, *a, **kw):
         h2d, d2h = a[-2], a[-1]
@@ -301,13 +321,13 @@ def timed_offload_run(args, policy, host_batches, B, T):
         orig_off(hm, *a, **kw)
         ev[1].record(h2d)
         ev[3].record(d2h)
-        spans.append((ev, 12 * hm.numel()))
-    z.ops.adamw_offload_bucket = timed_off
+        spans.append((ev, z.state_bytes(hm.numel(), optim)))
+    setattr(z.ops, entry, timed_off)
     try:
         run(1)
         torch.cuda.synchronize()
     finally:
-        z.ops.adamw_offload_bucket = orig_off
+        setattr(z.ops, entry, orig_off)
     streamed_bytes = sum(b for _, b in spans)
     h2d_ms = sum(ev[0].elapsed_time(ev[1]) for ev, _ in spans)
     d2h_ms = sum(ev[2].elapsed_time(ev[3]) for ev, _ in spans)
@@ -315,7 +335,7 @@ def timed_offload_run(args, policy, host_batches, B, T):
     pipeline_ms = first_h2d.elapsed_time(last_d2h)
     plain = plain_copy_gbs(opt.host_master[: min(opt.host_master.numel(), 1 << 28)])
     plain["both_at_once"] = concurrent_copy_gbs(opt.host_master[: min(opt.host_master.numel(), 1 << 28)])
-    ring_alone = ring_alone_gbs(opt)
+    ring_alone = ring_alone_gbs(opt) if optim == "adamw_torch" else None
     gbs = lambda b, t: b / (t * 1e-3) / 1e9 if t > 0 else None           # noqa: E731
     med = lambda xs: xs[len(xs) // 2] if xs else None                     # noqa: E731
     out = {
@@ -323,8 +343,10 @@ def timed_offload_run(args, policy, host_batches, B, T):
         "step0_loss": loss0, "ln2": math.log(2.0), "step0_ok": abs(loss0 - math.log(2.0)) < 1e-3,
         "ms_per_step": ms, "pairs_per_s": B / (ms * 1e-3),
         "device_free_before_optimizer_bytes": free, "activation_reserve_bytes": reserve,
-        "device_budget_bytes": opt.device_budget, "resident_bytes": 12 * opt.resident_elems,
-        "streamed_bytes": 12 * opt.streamed_elems, "pinned_host_bytes": opt.pinned_bytes,
+        "optim": optim, "device_budget_bytes": opt.device_budget,
+        "resident_bytes": sum(z.state_bytes(s1 - s0, optim) for (b, s0, s1, _), st in zip(opt.slices, opt._is_streamed)
+                              if not st),
+        "streamed_bytes": opt.pinned_bytes, "pinned_host_bytes": opt.pinned_bytes,
         "resident_buckets": len(opt.resident_names), "streamed_buckets": len(opt.streamed_names),
         "optimizer_setup_s": setup_s,
         "peak_device_allocated_bytes": peak_alloc, "peak_device_reserved_bytes": peak_reserved,
@@ -435,42 +457,187 @@ def config_d(args, tune_clip):
     return out
 
 
-def trained_tower_plan(args):
+def trained_tower_plan(args, optim="adamw_torch"):
     """The trained-tower recipe (--micro_pairs 1): the planner's numbers, then the run itself where MemAvailable holds
     the streamed state, otherwise the optimizer's refusal."""
     from rlaifv_b200.engine import DPOStepEngine
-    from rlaifv_b200.zero2 import (DEFAULT_SLOT_ELEMS, DEFAULT_SLOTS, DEVICE_MARGIN, HOST_MARGIN, STATE_BYTES_PER_ELEM,
-                                   offload_plan)
+    gc.collect()
+    torch.cuda.empty_cache()
+    policy = omni_policy(32, None, 1, args.max_len)
+    return planned_run(args, policy, omni_batches, bench.PROMPT_LEN + bench.RESP_LEN - 1 + policy.dims.num_query + 2,
+                       optim)
+
+
+def planned_run(args, policy, make_batches, T, optim="adamw_torch"):
+    """The planner's split for `policy` with micro-batches of one pair and the host memory it needs; then the timed run
+    where MemAvailable holds the streamed state, otherwise the optimizer's refusal."""
+    from rlaifv_b200.zero2 import (DEFAULT_SLOT_ELEMS, DEFAULT_SLOTS, DEVICE_MARGIN, HOST_MARGIN, offload_plan,
+                                   ring_bytes, ring_slot_elems, state_bytes)
     gc.collect()
     torch.cuda.empty_cache()
     B, micro = bench.PAIRS_PER_GPU, 1
-    policy = omni_policy(32, None, 1, args.max_len)
     sizes = [(b.name, b.size) for b in policy.trainable_buckets()]
     free = torch.cuda.mem_get_info()[0]
     reserve = policy.activation_reserve_bytes(micro, policy.dims.max_len)
-    ring = DEFAULT_SLOTS * 3 * min(DEFAULT_SLOT_ELEMS, max(n for _, n in sizes)) * 4
+    ring = ring_bytes(DEFAULT_SLOTS, ring_slot_elems(max(n for _, n in sizes), DEFAULT_SLOT_ELEMS, optim), optim)
     budget = free - reserve - ring - DEVICE_MARGIN
-    resident, streamed = offload_plan(sizes, budget)
+    resident, streamed = offload_plan(sizes, budget, optim)
     n_of = dict(sizes)
-    streamed_bytes = STATE_BYTES_PER_ELEM * sum(n_of[n] for n in streamed)
-    plan = {"micro_pairs": micro, "max_len": policy.dims.max_len, "trainable_elems": sum(n_of.values()),
+    streamed_bytes = sum(state_bytes(n_of[n], optim) for n in streamed)
+    plan = {"optim": optim, "micro_pairs": micro, "max_len": policy.dims.max_len, "trainable_elems": sum(n_of.values()),
             "device_free_before_optimizer_bytes": free, "activation_reserve_bytes": reserve,
-            "device_budget_bytes": budget, "resident_bytes": STATE_BYTES_PER_ELEM * sum(n_of[n] for n in resident),
+            "device_budget_bytes": budget, "resident_bytes": sum(state_bytes(n_of[n], optim) for n in resident),
             "streamed_bytes": streamed_bytes, "host_needed_bytes": streamed_bytes + HOST_MARGIN,
             "mem_available_bytes": mem_available(), "resident_buckets": len(resident), "streamed_buckets": len(streamed)}
-    try:
-        eng = DPOStepEngine(policy, offload_optimizer=True, micro_pairs=micro, batch_pairs=B)
-    except MemoryError as e:
-        plan["refused"] = str(e)
-        return plan
-    eng.opt.close()
-    del eng
-    gc.collect()
     a = argparse.Namespace(**vars(args))
     a.micro_pairs = micro
-    T = bench.PROMPT_LEN + bench.RESP_LEN - 1 + policy.dims.num_query + 2
-    plan["run"] = timed_offload_run(a, policy, omni_batches(policy, B), B, T)
+    try:        # the engine's optimizer refuses before it pins anything when MemAvailable is too small
+        plan["run"] = timed_offload_run(a, policy, make_batches(policy, B), B, T, optim)
+    except MemoryError as e:
+        plan["refused"] = str(e)
     return plan
+
+
+# ---- AdamW with blockwise 8-bit moments (--optim adamw_8bit) -----------------------------------------------------------
+def kernel_throughput(n=1 << 30, reps=20):
+    """rlaifv_adamw8bit_step against the fp32 rlaifv_adamw_step (adamw_kernel) on one n-element shard, CUDA events.
+    Algorithmic bytes per element: fp32 master read + write 8, bf16 grad 2 and param 2, codes read + write 4 (8-bit:
+    16 B + 16 B per 256 elements for the absmax) or fp32 m and v read + write 16 (fp32: 28 B)."""
+    from rlaifv_b200 import ops
+    from rlaifv_b200.zero2 import dynamic_map
+    g = torch.Generator(device="cuda").manual_seed(0)
+    grad = (torch.randn(n, generator=g, device="cuda") * 1e-3).bfloat16()
+    param = torch.empty(n, dtype=torch.bfloat16, device="cuda")
+    master = torch.randn(n, generator=g, device="cuda") * 0.02
+    out = {"elements": n, "reps": reps}
+    nb = (n + 255) // 256
+    state8 = [torch.full((n,), 127, dtype=torch.uint8, device="cuda"), torch.zeros(n, dtype=torch.uint8, device="cuda"),
+              torch.zeros(nb, device="cuda"), torch.zeros(nb, device="cuda")]
+    maps = [dynamic_map(True).cuda(), dynamic_map(False).cuda()]
+    run8 = lambda st: ops.adamw8bit_step(master, *state8, grad, param, n, *maps, 1e-6, 0.9, 0.999, 1e-8, 0.01, st)  # noqa
+    for name, fn, bpe in (("adamw_8bit", run8, 16 + 16 / 256), ("adamw_torch", None, 28)):
+        if fn is None:
+            m, v = torch.zeros_like(master), torch.zeros_like(master)
+            fn = lambda st: ops.adamw_step(master, m, v, grad, param, 1e-6, 0.9, 0.999, 1e-8, 0.01, st)  # noqa
+        for st in range(1, 4):
+            fn(st)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for st in range(4, 4 + reps):
+            fn(st)
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / reps
+        out[name] = {"ms": ms, "bytes_per_elem": bpe, "gbs": bpe * n / (ms * 1e-3) / 1e9}
+        if fn is not run8:
+            del m, v
+    return out
+
+
+def identity8(layers):
+    """Three steps with 8-bit moments on the device, then from the same seed offloaded with a mixed and an all-streamed
+    split: metrics, bf16 parameters and every state tensor bit for bit."""
+    from rlaifv_b200.zero2 import state_bytes, state_parts
+    B, micro = 4, 2
+    batches = [bench.synthetic_batch(0, s, B) for s in range(3)]
+    keys = [k for k, _, _ in state_parts("adamw_8bit")]
+    results, splits = {}, {}
+    for mode in ("device", "mixed", "all_streamed"):
+        budget = None
+        if mode == "mixed":
+            budget = sum(state_bytes(sizes[n], "adamw_8bit") for n in ("embed", "projector", "layer0", "layer1"))
+        elif mode == "all_streamed":
+            budget = 0
+        eng = make_engine(layers, micro, offload_budget=budget, offload=budget is not None, optim="adamw_8bit")
+        if mode == "device":
+            sizes = {b.name: b.size for b in eng.policy.trainable_buckets()}
+            add_reference_logps(eng.policy, batches, B, micro)
+        metrics = [eng.train_step(hb).clone() for hb in batches]
+        eng.opt.wait_all()
+        torch.cuda.synchronize()
+        sd = eng.opt.state_dict()
+        results[mode] = {"metrics": torch.stack(metrics).cpu(), "params": eng.policy.store.flat.cpu(),
+                         **{k: sd[k].cpu() for k in keys}}
+        if budget is not None:
+            splits[mode] = {"resident": eng.opt.resident_names, "streamed": len(eng.opt.streamed_names)}
+            eng.opt.close()
+        del eng, sd
+        gc.collect()
+        torch.cuda.empty_cache()
+    d = results["device"]
+    out = {"layers": layers, "pairs": B, "micro_pairs": micro, "steps": 3}
+    for mode in ("mixed", "all_streamed"):
+        o = results[mode]
+        out[mode] = {**splits[mode], **{k + "_identical": bool(torch.equal(d[k], o[k])) for k in d}}
+    return out
+
+
+def loss_trajectory(steps=20, layers=2):
+    """7B widths at `layers` layers, `steps` steps of each optimizer from one seed on bench.py's inputs (4 pairs,
+    micro-batches of 2, lr 5e-7 as in the recipe): the largest |delta loss| over the steps and the relative difference
+    of the fp32 master weights at the end."""
+    B, micro = 4, 2
+    batches = [bench.synthetic_batch(0, s, B) for s in range(steps)]
+    res = {}
+    for optim in ("adamw_torch", "adamw_8bit"):
+        eng = make_engine(layers, micro, optim=optim)
+        if optim == "adamw_torch":
+            add_reference_logps(eng.policy, batches, B, micro)
+            m0 = eng.opt.master.cpu()
+        losses = [float(eng.train_step(hb)[0]) for hb in batches]
+        eng.opt.wait_all()
+        torch.cuda.synchronize()
+        res[optim] = (losses, eng.opt.master.cpu())
+        del eng
+        gc.collect()
+        torch.cuda.empty_cache()
+    (l32, m32), (l8, m8) = res["adamw_torch"], res["adamw_8bit"]
+    return {"layers": layers, "steps": steps, "pairs": B, "lr": 5e-7, "loss_adamw_torch": l32, "loss_adamw_8bit": l8,
+            "max_abs_delta_loss": max(abs(a - b) for a, b in zip(l32, l8)),
+            "master_rel_diff": float((m8 - m32).norm() / m32.norm()),
+            "master_rel_diff_of_update": float((m8 - m32).norm() / (m32 - m0).norm())}
+
+
+def llava13b_full_ft(args):
+    """13B full fine-tuning with 8-bit moments: 8 pairs of bench.py's T in micro-batches of one pair, model_max_length
+    2048, seeded weights; measured where MemAvailable holds the streamed state, otherwise the refusal."""
+    from rlaifv_b200.model import LlavaDims, LlavaDPOPolicy
+    gc.collect()
+    torch.cuda.empty_cache()
+    dims = LlavaDims(hidden_size=5120, intermediate_size=13824, num_layers=40, num_heads=40, max_len=2048)
+    policy = LlavaDPOPolicy(dims, torch.device("cuda", 0), seed=0)
+    T = bench.PROMPT_LEN + bench.RESP_LEN - 1 + dims.num_patches
+    return planned_run(args, policy, lambda pol, B: [bench.synthetic_batch(0, s, B) for s in range(2)], T,
+                       "adamw_8bit")
+
+
+def adamw8bit_main(args, line):
+    path = os.path.join(args.out, "offload_step_8bit.json")
+    line["mem_available_bytes"] = mem_available()
+
+    def dump(key):
+        print(json.dumps({key: line[key]}), flush=True)
+        with open(path, "w") as f:
+            json.dump(line, f, indent=1)
+    legs = [("kernel", args.skip_kernel, kernel_throughput),
+            ("identity", args.skip_identity, lambda: identity8(args.identity_layers)),
+            ("loss_trajectory", args.skip_trajectory, loss_trajectory),
+            ("config_b", args.skip_config_b, lambda: [config_b(args, optim) for optim in
+                                                      ("adamw_torch", "adamw_8bit", "adamw_torch", "adamw_8bit")]),
+            ("llava13b_full_ft", args.skip_13b, lambda: llava13b_full_ft(args)),
+            ("omnilmm_trained_tower", args.skip_trained_tower, lambda: trained_tower_plan(argparse.Namespace(**dict(vars(args), max_len=1024)),
+                                                                     "adamw_8bit"))]
+    for key, skip, fn in legs:
+        if skip:
+            continue
+        try:
+            line[key] = fn()
+        except torch.OutOfMemoryError as e:
+            line[key] = {"out_of_memory": str(e).splitlines()[0]}
+        gc.collect()
+        torch.cuda.empty_cache()
+        dump(key)
+    print(json.dumps(line), flush=True)
 
 
 def omnilmm_main(args, line):
@@ -502,6 +669,8 @@ def main(argv=None):
     line = {"gpu": name, "power_limit": power}
     if args.omnilmm:
         return omnilmm_main(args, line)
+    if args.optim == "adamw_8bit":
+        return adamw8bit_main(args, line)
     if not args.skip_identity:
         line["identity"] = identity(args.identity_layers)
         print(json.dumps({"identity": line["identity"]}), flush=True)
