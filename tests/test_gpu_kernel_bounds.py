@@ -29,7 +29,7 @@ LOG2E = 1.0 / math.log(2.0)
 
 ATT_TILE = 128             # attention_fwd_kernel: KV tile rows
 LAZY_MAX = 8.0             # ... the running max moves only when a tile's max beats it by more than this (log2 units)
-ACC = 2.0 ** -14           # GEMM: fp32 accumulation over K, relative to (|A| |B|)_ij
+ACC = 2.0 ** -14           # GEMM: fp32 accumulation over K, relative to (|A| |B|)_ij (acc_term: its floor)
 ACT_SLOPE = 1.13           # max |d/dx| of GELU(erf) and of quick-GELU x * sigmoid(1.702 x)
 H100_SMS = 132
 
@@ -76,21 +76,56 @@ def assert_within(name, got, ref, bound):
 
 
 # ------------------------------------------------------------------------------------------------ GEMM
-def gemm_ref(a, b, a_mn, b_mn):
+def acc_term(k=0):
+    """Relative error of the fp32 wgmma accumulator after a contraction of depth k, as a multiple of (|A| |B|)_ij.
+
+    The products of two bf16 values are exact in fp32. Each 16-deep wgmma step adds 16 of them to the accumulator;
+    take its error as at most two fp32 units in the last place (2^-22: the alignment of the addends and the rounding
+    of the sum, either of which may truncate) of the magnitude summed so far, which (|A| |B|)_ij bounds. Over
+    ceil(k / 16) steps the errors add up to ceil(k / 16) 2^-22 (|A| |B|)_ij, Higham's recursive-summation bound
+    (Accuracy and Stability of Numerical Algorithms, 2nd ed., section 4.2) with one term per step. Zero-filled steps
+    past K add exact zeros. That passes the fixed 2^-14 above k = 4096: at the step's deepest launch (gate|up dgrad of
+    LLaVA-1.5-13B, k = 27 648) it is 1728 x 2^-22 = 2^-11.2, so the fixed term could not be shown to hold there. For
+    k <= 4096 the term stays 2^-14, so the bound of every shallower case is unchanged."""
+    return max(ACC, math.ceil(k / 16) * 2.0 ** -22)
+
+
+def gemm_ref(a, b, a_mn, b_mn, *, a2=None, b2=None, k2=0, r=0, n_sub=0, rows=None, cols=None):
     """op(a) @ op(b)^T in fp64, and the same product of absolute values (a_mn: a stored [K, M]; b_mn: b stored
-    [K, N])."""
-    x = (a.t() if a_mn else a).to(F64)
-    y = (b if b_mn else b.t()).to(F64)
-    return x @ y, x.abs() @ y.abs()
+    [K, N]).
+
+    Second source (gemm.cu GemmSecondSource): + a2[:, koff(n) : koff(n) + k2] @ op(b2)^T, a2 stored [M, *] (K-major),
+    b2 in b's layout ([k2, N] when b_mn), koff(n) = (n // n_sub) * r for output column n (0 when n_sub == 0): the
+    kernel's koff = (n0 / n_sub) * r is the same for every column of a tile since the tile divides n_sub. Columns of
+    a2 past its extent read as zero, as TMA fills them. rows / cols (slices): only that block of the output."""
+    rows = rows if rows is not None else slice(None)
+    cols = cols if cols is not None else slice(None)
+    x = (a.t() if a_mn else a)[rows].to(F64)
+    y = (b if b_mn else b.t())[:, cols].to(F64)
+    c, mag = x @ y, x.abs() @ y.abs()
+    if a2 is None:
+        return c, mag
+    assert not a_mn, "the second source is instantiated for K-major A only"
+    y2 = (b2 if b_mn else b2.t())[:, cols]
+    n = torch.arange(b.shape[1] if b_mn else b.shape[0])[cols]
+    koff = (n // n_sub) * r if n_sub else torch.zeros_like(n)
+    for k0 in koff.unique().tolist():
+        j = (koff == k0).nonzero().squeeze(1).to(y2.device)
+        x2 = a2[rows, k0:k0 + k2].to(F64)
+        w2 = y2[:x2.shape[1], j].to(F64)
+        c[:, j] += x2 @ w2
+        mag[:, j] += x2.abs() @ w2.abs()
+    return c, mag
 
 
-def epilogue_ref(acc, mag, *, alpha=1.0, bias=None, act=0, residual=None, old=None):
+def epilogue_ref(acc, mag, *, k=0, alpha=1.0, bias=None, act=0, residual=None, old=None):
     """gemm.cu epilogue_pair in fp64, rounding to bf16 where the kernel rounds. Returns (reference, bound).
 
-    The bound starts at the accumulation term ACC * |A||B| and gains one bf16 ulp at every rounding point (the kernel
-    and the reference may round a value to neighbouring bf16 numbers), carried through the later steps. Without an
-    epilogue it is ulp(C64) + 2^-14 (|A||B|), the ulp taken at |C64| plus the accumulation term."""
-    v, e = acc, ACC * mag
+    The bound starts at the accumulation term acc_term(k) * |A||B| (k: the contraction depth, K + K2 with a second
+    source) and gains one bf16 ulp at every rounding point (the kernel and the reference may round a value to
+    neighbouring bf16 numbers), carried through the later steps. Without an epilogue it is ulp(C64) + acc_term(k)
+    (|A||B|), the ulp taken at |C64| plus the accumulation term."""
+    v, e = acc, acc_term(k) * mag
 
     def rnd(v, e):
         return bf16(v), e + ulp_bf16(v.abs() + e)
@@ -116,18 +151,19 @@ def epilogue_ref(acc, mag, *, alpha=1.0, bias=None, act=0, residual=None, old=No
 
 def pow2_rows(x, gen, span=6):
     """x with each row scaled by 2^u, u uniform in [-span, span] (exact in bf16)."""
-    u = torch.randint(-span, span + 1, (x.shape[0], 1), generator=gen).to(x.dtype)
+    u = torch.randint(-span, span + 1, (x.shape[0], 1), generator=gen, device=gen.device).to(x)
     return x * torch.exp2(u)
 
 
 def gemm_operand(rows, k, mn, gen, pad=0, device=DEV):
     """Logical [rows, k] bf16 operand with power-of-two row scales; mn: stored transposed ([k, rows]). pad > 0: a
-    column block (at column 8) of a wider buffer whose other columns are NaN, so the row stride exceeds the extent."""
-    x = pow2_rows(torch.randn(rows, k, generator=gen, dtype=F64), gen).to(BF)
+    column block (at column 8) of a wider buffer whose other columns are NaN, so the row stride exceeds the extent.
+    The values are drawn on gen's device (a CUDA generator keeps large operands off the host)."""
+    x = pow2_rows(torch.randn(rows, k, generator=gen, dtype=F64, device=gen.device), gen).to(BF)
     st = x.t().contiguous() if mn else x
     if not pad:
         return st.to(device)
-    buf = torch.full((st.shape[0], st.shape[1] + pad), float("nan"), dtype=BF)
+    buf = torch.full((st.shape[0], st.shape[1] + pad), float("nan"), dtype=BF, device=gen.device)
     buf[:, 8:8 + st.shape[1]] = st
     return buf.to(device)[:, 8:8 + st.shape[1]]
 

@@ -228,11 +228,13 @@ def expf_fast_rel(x):
     return (2 + torch.floor((1.173 * x).abs())) * ULP1
 
 
-def sigmoid_err(g):
+def sigmoid_err(g, fast_div=False):
     """sg = 1 / (1 + __expf(-g)): __expf's error scaled by E / (1 + E) <= 1, the add and the division (gamma_2), and
-    the flush / overflow floor (for g < -88.7 __expf(-g) is inf and sg = 0, while sigmoid(g) < 2^-128)."""
+    the flush / overflow floor (for g < -88.7 __expf(-g) is inf and sg = 0, while sigmoid(g) < 2^-128). fast_div:
+    the division is __fdividef (2 ulp, i.e. 4 u, instead of correctly rounded; it returns 0 for a divisor past 2^126,
+    inside the same floor)."""
     s = torch.sigmoid(g)
-    return s, s * (expf_fast_rel(-g) + gam(2)) * (1 + 1e-6) + FTZ
+    return s, s * (expf_fast_rel(-g) + (gam(5) if fast_div else gam(2))) * (1 + 1e-6) + FTZ
 
 
 def swiglu_fwd_ref(gu):
@@ -249,17 +251,22 @@ def swiglu_fwd_ref(gu):
     return act, rounded(act, u.abs() * e_b)
 
 
-def swiglu_bwd_ref(gu, dact):
+def swiglu_bwd_ref(gu, dact, e_dact=None, fast_div=False):
     """sg as in sigmoid_err; du = d * fl(g sg); dg = fl(fl(d u) ... : (d u) exact, times
-    fl(sg * fma(g, fl(1 - sg), 1)), each step one rounding on its magnitude."""
+    fl(sg * fma(g, fl(1 - sg), 1)), each step one rounding on its magnitude.
+
+    e_dact: the kernel's d may differ from dact by this much (the GEMM's fused form rounds its fp32 accumulator to bf16
+    for d, and dact is then the fp64 product): |d| + e_dact stands for |d| in every rounding term, and e_dact times the
+    computed factors (silu, u silu') is added. fast_div: sigmoid_err's __fdividef (gemm.cu swiglu_bwd_pair)."""
     gu, d = gu.to(F64), dact.to(F64)
     F = gu.shape[1] // 2
     g, u = gu[:, :F], gu[:, F:]
-    s, e_s = sigmoid_err(g)
+    s, e_s = sigmoid_err(g, fast_div)
     ag = g.abs()
+    ad = d.abs() if e_dact is None else d.abs() + e_dact
     e_silu = ag * e_s + U * ag * (s + e_s)
     du = d * g * s
-    e_du = d.abs() * e_silu + U * d.abs() * ag * (s + e_s)
+    e_du = ad * e_silu + U * ad * ag * (s + e_s)
     one_m = 1 - s
     e_t1 = e_s + U * (one_m + e_s)
     A2 = 1 + ag * one_m
@@ -267,7 +274,10 @@ def swiglu_bwd_ref(gu, dact):
     e_t3 = e_s * (A2 + e_t2) + s * e_t2 + U * (s + e_s) * (A2 + e_t2)
     dgu = d * u
     dg = dgu * s * (1 + g * one_m)
-    e_dg = dgu.abs() * e_t3 + U * dgu.abs() * (s * A2 + e_t3)
+    e_dg = ad * u.abs() * e_t3 + U * ad * u.abs() * (s * A2 + e_t3)
+    if e_dact is not None:
+        e_du = e_du + e_dact * ag * (s + e_s)
+        e_dg = e_dg + e_dact * u.abs() * s * A2
     return (dg, rounded(dg, e_dg)), (du, rounded(du, e_du))
 
 

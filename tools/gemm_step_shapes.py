@@ -43,13 +43,15 @@ PAIRS, MICRO_PAIRS = 8, 4   # bench.py: pairs per step and per micro-batch
 STALL_FIELDS = ("ctas", "tiles", "cons_total", "cons_full_wait", "cons_epilogue", "prod_total", "prod_empty_wait")
 
 
-def shape_names(H, F):
+def shape_names(H, F, lora=True):
     """Names of the frozen-base shapes: (function, N, K) -> name; N / K are the launch's output columns / first-source
-    depth. The two H x H launches are told apart by the layout of B."""
-    return {("gemm_dual", 3 * H, H): "qkv forward", ("gemm_dual", H, H, False): "o forward",
-            ("gemm_dual", 2 * F, H): "gate|up forward", ("gemm_dual", H, F): "down forward",
-            ("gemm_swiglu_bwd", F, H): "down dgrad (SwiGLU bwd)", ("gemm_dual", H, 2 * F): "gate|up dgrad",
-            ("gemm_dual", H, H, True): "o dgrad", ("gemm_dual", H, 3 * H): "qkv dgrad"}
+    depth. The two H x H launches are told apart by the layout of B. Full fine-tuning (lora=False) runs the same
+    shapes as plain gemm launches, the fused SwiGLU backward included."""
+    dual = "gemm_dual" if lora else "gemm"
+    return {(dual, 3 * H, H): "qkv forward", (dual, H, H, False): "o forward",
+            (dual, 2 * F, H): "gate|up forward", (dual, H, F): "down forward",
+            ("gemm_swiglu_bwd", F, H): "down dgrad (SwiGLU bwd)", (dual, H, 2 * F): "gate|up dgrad",
+            (dual, H, H, True): "o dgrad", (dual, H, 3 * H): "qkv dgrad"}
 
 
 def parse_args(argv=None):
@@ -135,8 +137,9 @@ def card_info():
     return info
 
 
-def record_step_calls(dims):
-    """One LoRA-DPO training step of a one-layer policy at the benchmark's batch: every GEMM call with its tensors."""
+def record_step_calls(dims, lora=True):
+    """One DPO training step of a one-layer policy at the benchmark's batch, LoRA(r=64) or (lora=False) full
+    fine-tuning: every GEMM call with its tensors."""
     import torch
     import bench
     from rlaifv_b200 import ops
@@ -145,7 +148,8 @@ def record_step_calls(dims):
     policy = LlavaDPOPolicy(LlavaDims(num_layers=1, hidden_size=dims["hidden_size"],
                                       intermediate_size=dims["intermediate_size"], num_heads=dims["num_heads"]),
                             torch.device("cuda", 0), seed=0)
-    policy.enable_lora(r=64, alpha=16)
+    if lora:
+        policy.enable_lora(r=64, alpha=16)
     engine = DPOStepEngine(policy, lr=1e-5, weight_decay=0.01, total_steps=2672, micro_pairs=MICRO_PAIRS)
     hb = bench.synthetic_batch(0, 0, PAIRS)
     batch = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in hb.items()}
@@ -199,12 +203,12 @@ def describe(name, a, kw, r):
     return (name, t_sig, kw_sig), d
 
 
-def shape_name(d, dims):
+def shape_name(d, dims, lora=True):
     H = dims["hidden_size"]
     key = (d["fn"], d["N"], d["K"])
-    if d["fn"] == "gemm_dual" and d["N"] == d["K"] == H:
+    if d["fn"] != "gemm_swiglu_bwd" and d["N"] == d["K"] == H:
         key = key + (d["B"] == "MN",)
-    return shape_names(H, dims["intermediate_size"]).get(key)
+    return shape_names(H, dims["intermediate_size"], lora).get(key)
 
 
 def is_adapter(d, r=64):
