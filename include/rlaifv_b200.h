@@ -367,6 +367,32 @@ int rlaifv_adamw8bit_offload_bucket(float* host_master, uint8_t* host_code_m, ui
                                     int n_slots, long long slot_elems, float lr, float beta1, float beta2, float eps,
                                     float weight_decay, int step, void* stream, void* h2d_stream, void* d2h_stream);
 
+/* ---- FP8 (e4m3) frozen base of LoRA training (DESIGN.md §3 "FP8 frozen base"). Format: a tile (1 x 128 of an
+ * operand row, or a 128 x 128 block of a weight) with amax = max|x| has the scale s = 2^e, e the smallest integer with
+ * amax <= 448 * 2^e clamped to [-126, 127] (s = 1 for amax = 0), and the codes RNE_e4m3(x / s); x / s is exact and
+ * never saturates. oracle/fp8_oracle.py is the reference. K and N must be multiples of 128.
+ * rlaifv_quant_fp8_rows: x [M, K] bf16 (row stride ldx) -> codes q [M, K] (ldq bytes, multiple of 16) and the row
+ * scales s [K / 128][ld_s] fp32 (ld_s >= M, multiple of 4: the rows of one K-block are contiguous). */
+int rlaifv_quant_fp8_rows(const void* x, long long ldx, void* q, long long ldq, float* s, long long ld_s, int M, int K,
+                          void* stream);
+/* W [N, K] bf16 -> W codes q [N, K] (ldq), W^T codes qt [K, N] (ldt; the byte-for-byte transpose of q) and the block
+ * scales s [N / 128][ld_s] (ld_s >= K / 128). Once per weight, when the model loads. */
+int rlaifv_quant_fp8_blocks(const void* w, long long ldw, void* q, long long ldq, void* qt, long long ldt, float* s,
+                            long long ld_s, int N, int K, void* stream);
+/* C[m, n] = sum_kb sa[kb][m] * sb(n / 128, kb) * sum_{k in kb} A[m, k] * B[n, k] over e4m3 codes (A [M, K], lda
+ * bytes; B [N, K], ldb bytes), each 128-deep K-block accumulated apart and promoted in fp32, then
+ * + A2[:, koff : koff + K2] * B2^T (bf16, as rlaifv_gemm_bf16_dual: koff = (n0 / n_sub) * r, n_sub % 128 == 0),
+ * then one of: C = bf16(acc); C = bf16(bf16(acc) + residual) (residual [M, ldr]); glu != NULL: the SwiGLU-backward
+ * epilogue of rlaifv_gemm_bf16_swiglu_bwd (N = F, glu = [gate | up] [M, ld_glu], C = d[gate | up] [M, 2F]).
+ * sb: the block scales of a weight W [N_w, K_w] ([N_w / 128][K_w / 128]). b_t = 0: B is W (forward), sb(nb, kb) =
+ * sb[nb * K / 128 + kb]; b_t = 1: B is W^T (dgrad), sb(nb, kb) = sb[kb * N / 128 + nb], and B2 is MN-major
+ * ([K2, N], as rlaifv_gemm_bf16_dual with b_mn_major = 1). C and the residual are 16-byte aligned, ldc and ldr
+ * multiples of 8; C may be a column block of a wider buffer. */
+int rlaifv_gemm_fp8(const void* A, long long lda, const float* sa, long long ld_sa, const void* B, long long ldb,
+                    const float* sb, int b_t, const void* A2, long long lda2, const void* B2, long long ldb2, int K2,
+                    int r, int n_sub, void* C, long long ldc, int M, int N, int K, const void* residual, long long ldr,
+                    const void* glu, long long ld_glu, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

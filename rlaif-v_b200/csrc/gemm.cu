@@ -561,6 +561,180 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (CL == 2) cluster_sync_all();    // the peer may still multicast into / arrive on this CTA's shared memory
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// FP8 frozen-base GEMM (DESIGN.md §3 "FP8 frozen base"): C = sum_kb sa[m, kb] * sb[n / 128, kb] * (qa[m, kb] . qb[n, kb])
+// over e4m3 codes in 128-deep K-blocks, then the optional bf16 second source, then the plain, residual or
+// SwiGLU-backward staged epilogue. One SWIZZLE_128B row holds 128 e4m3, so an FP8 stage (128 x 128 bytes of A and of
+// B) has the byte layout of a bf16 stage of 64 K and the same descriptor stepping (one k32 step = 32 bytes); the ring,
+// the producer protocol and the staging atoms are those of gemm_bf16_kernel at tile 128 x 128.
+// The tensor cores accumulate FP8 products at a reduced, undocumented precision, so each K-block goes into its own
+// partial accumulator (scale-d = 0 on its first k32 step) and is promoted into the fp32 accumulator with one FMA by
+// the exact power-of-two product of its two scales. Two 64-register accumulators per math thread.
+constexpr int FP8_BK = 128;     // e4m3 per K-block: one 128-byte swizzled row, one scale per row / per weight block
+
+struct Fp8Scales {
+  const float* sa;     // row scales of A: [K / 128][ld_sa], row m of K-block kb at sa[kb * ld_sa + m]
+  long long ld_sa;
+  const float* sb;     // block scales of B: output block nb, K-block kb at sb[nb * sb_n + kb * sb_k]
+  int sb_n, sb_k;
+};
+
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
+}
+
+// tmA / tmB: e4m3 codes as {K, rows} bytes in 128 x 128 boxes; tmA2 / tmB2: the bf16 second source as in
+// gemm_bf16_kernel (B2 MN-major when B2_MN); tmC / tmR as in the staged bf16 kernel. K % 128 == 0, N % 128 == 0.
+template <int EPI, bool B2_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
+                int M, int N, int K, GemmSecondSource src2, Fp8Scales sc, GemmEpilogue epi) {
+  constexpr int BN = 128;
+  using Cfg = GemmCfg<BN, EPI, true>;
+  constexpr int STAGES = Cfg::STAGES;
+  static_assert(Cfg::A_BYTES == GEMM_BM * FP8_BK && Cfg::B_BYTES == BN * FP8_BK, "an e4m3 stage fills a bf16 slot");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(staging + 2 * Cfg::WG_STAGING_BYTES);
+  uint64_t* empty = full + STAGES;
+  uint64_t* ebar = empty + STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
+  const int num_m = (M + GEMM_BM - 1) / GEMM_BM;
+  const int num_n = N / BN;
+  const int num_tiles = num_m * num_n;
+  const int num_k1 = K / FP8_BK;
+  const int num_k = num_k1 + (src2.K2 + GEMM_BK - 1) / GEMM_BK;
+  const bool n_grouped = (epi.l2 & 0x40) != 0;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    if (src2.K2 > 0) {
+      tma_prefetch_desc(&tmA2);
+      tma_prefetch_desc(&tmB2);
+    }
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 8);
+    }
+    for (int i = 0; i < 2 * Cfg::SLOTS; ++i) mbar_init(&ebar[i], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ------------------------------ TMA producer ------------------------------
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      const uint64_t pol_a = l2_policy(epi.l2 & 3), pol_b = l2_policy((epi.l2 >> 2) & 3);
+      int s = 0;
+      uint32_t ph = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        int m_blk, n_blk;
+        tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, n_grouped);
+        const int m0 = m_blk * GEMM_BM, n0 = n_blk * BN;
+        for (int kb = 0; kb < num_k; ++kb) {
+          mbar_wait(&empty[s], ph ^ 1);
+          uint8_t* a_dst = smem + s * Cfg::STAGE_BYTES;
+          uint8_t* b_dst = a_dst + Cfg::A_BYTES;
+          mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
+          if (kb < num_k1) {
+            tma_load_2d_hint(a_dst, &tmA, &full[s], kb * FP8_BK, m0, pol_a);
+            tma_load_2d_hint(b_dst, &tmB, &full[s], kb * FP8_BK, n0, pol_b);
+          } else {
+            const int kB = (kb - num_k1) * GEMM_BK;
+            const int kA = kB + (src2.n_sub > 0 ? (n0 / src2.n_sub) * src2.r : 0);
+            tma_load_2d_hint(a_dst, &tmA2, &full[s], kA, m0, pol_a);
+            if (B2_MN) {
+#pragma unroll
+              for (int a = 0; a < BN / 64; ++a)
+                tma_load_2d_hint(b_dst + a * ATOM_BYTES, &tmB2, &full[s], n0 + a * 64, kB, pol_b);
+            } else {
+              tma_load_2d_hint(b_dst, &tmB2, &full[s], kB, n0, pol_b);
+            }
+          }
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ------------------------------ MMA, promotion + epilogue: 64 rows per warpgroup ------------------------------
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;
+    const int g = lane >> 2;
+    float acc[BN / 2], part[BN / 2];
+    int s = 0;
+    uint32_t ph = 0;             // bit 0: parity of the ring's `full` barriers; bits 1.. those of the staging slots
+    const bool leader = (threadIdx.x & 127) == 0;
+    StagedEpi se;
+    se.slots = smem_u32(staging + cw * Cfg::WG_STAGING_BYTES);
+    se.bar = smem_u32(ebar + cw * Cfg::SLOTS);
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      int m_blk, n_blk;
+      tile_coords(t, num_m, num_n, epi.group_m, m_blk, n_blk, n_grouped);
+      se.row0 = m_blk * GEMM_BM + cw * 64;
+      se.n0 = n_blk * BN;
+      if constexpr (EPI != EPI_PLAIN) {
+        if (leader) staged_prefetch<EPI, BN, Cfg>(se, &tmR, M, N);
+      }
+      const int r0 = se.row0 + (warp & 3) * 16 + g, r1 = r0 + 8;   // this thread's two accumulator rows
+      const float* sa0 = sc.sa + r0;
+      const float* sb = sc.sb + (long long)n_blk * sc.sb_n;
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < num_k; ++kb) {
+        const bool fp8 = kb < num_k1;
+        // scales first: the loads are in flight while the stage's MMAs run (rows past M have zero codes)
+        float f0 = 0.f, f1 = 0.f;
+        if (fp8) {
+          const float b = __ldg(sb + (long long)kb * sc.sb_k);
+          const long long o = (long long)kb * sc.ld_sa;
+          f0 = r0 < M ? __ldg(sa0 + o) * b : 0.f;
+          f1 = r1 < M ? __ldg(sa0 + o + 8) * b : 0.f;
+        }
+        mbar_wait(&full[s], ph & 1);
+        const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * ATOM_BYTES;
+        const uint32_t b_addr = smem_u32(smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+        if (fp8) {
+          reg_fence(part);
+          wgmma_fence();
+#pragma unroll
+          for (int k32 = 0; k32 < FP8_BK / 32; ++k32)
+            wgmma_m64n128k32_e4m3(part, desc_kmajor(a_addr, k32), desc_kmajor(b_addr, k32), k32 > 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(part);
+          if (lane == 0) mbar_arrive(&empty[s]);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = fmaf(part[i], (i & 2) ? f1 : f0, acc[i]);
+        } else {
+          reg_fence(acc);
+          wgmma_fence();
+          gemm_mma_stage<false, B2_MN, BN>(acc, a_addr, b_addr, 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(acc);
+          if (lane == 0) mbar_arrive(&empty[s]);
+        }
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      epilogue_staged<EPI, BN, Cfg>(acc, se, ph, &tmC, &tmR, M, N, leader, 1 + cw);
+    }
+    if (leader) tma_store_wait_all<0>();   // the slots must outlive the bulk stores that read them
+  }
+}
+
 struct GemmLaunch {
   CUtensorMap tmA, tmB, tmA2, tmB2, tmC, tmR;
   int M, N, K;
@@ -907,4 +1081,102 @@ extern "C" int rlaifv_gemm_bf16_dual(const void* A, long long lda, int a_mn_majo
   B200_REQUIRE(K2 > 0 && A2 && B2, "gemm_dual: second source missing");
   return gemm_impl(A, lda, a_mn_major, B, ldb, b_mn_major, C, ldc, M, N, K, bias, residual, ldr, act, accumulate, 0,
                    1.0f, stream, A2, lda2, B2, ldb2, K2, r, n_sub);
+}
+
+template <int EPI, bool B2_MN>
+static int launch_fp8(const GemmLaunch& L, const Fp8Scales& sc) {
+  using Cfg = GemmCfg<128, EPI, true>;
+  auto kern = gemm_fp8_kernel<EPI, B2_MN>;
+  B200_CHECK_CUDA(configure_smem_once((const void*)kern, (int)Cfg::SMEM_BYTES));
+  static int slots_per_device[64] = {};
+  int dev = 0;
+  B200_CHECK_CUDA(cudaGetDevice(&dev));
+  int& slots = slots_per_device[dev & 63];
+  if (slots == 0) slots = resident_clusters(kern, 1, (int)Cfg::SMEM_BYTES);
+  const int num_tiles = ((L.M + GEMM_BM - 1) / GEMM_BM) * (L.N / 128);
+  kern<<<num_tiles < slots ? num_tiles : slots, GEMM_THREADS, Cfg::SMEM_BYTES, L.stream>>>(
+      L.tmA, L.tmB, L.tmA2, L.tmB2, L.tmC, L.tmR, L.M, L.N, L.K, L.src2, sc, L.epi);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int rlaifv_gemm_fp8(const void* A, long long lda, const float* sa, long long ld_sa, const void* B,
+                               long long ldb, const float* sb, int b_t, const void* A2, long long lda2, const void* B2,
+                               long long ldb2, int K2, int r, int n_sub, void* C, long long ldc, int M, int N, int K,
+                               const void* residual, long long ldr, const void* glu, long long ld_glu, void* stream) {
+  B200_REQUIRE(A && B && sa && sb && C, "gemm_fp8: null operand");
+  B200_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: empty problem M=%d N=%d K=%d", M, N, K);
+  B200_REQUIRE(N % 128 == 0 && K % 128 == 0, "gemm_fp8: N (%d) and K (%d) must be multiples of 128", N, K);
+  B200_REQUIRE(lda >= K && ldb >= K && lda % 16 == 0 && ldb % 16 == 0,
+               "gemm_fp8: code row strides (lda %lld, ldb %lld) must cover K and be multiples of 16 bytes", lda, ldb);
+  B200_REQUIRE(ld_sa >= M && ld_sa % 4 == 0, "gemm_fp8: ld_sa (%lld) must be >= M (%d) and a multiple of 4", ld_sa, M);
+  B200_REQUIRE(((uintptr_t)sa & 15) == 0 && ((uintptr_t)sb & 3) == 0, "gemm_fp8: scales misaligned");
+  B200_REQUIRE(ldc % 8 == 0 && ((uintptr_t)C & 15) == 0, "gemm_fp8: C must be 16-byte aligned, ldc a multiple of 8");
+  B200_REQUIRE(!(glu && residual), "gemm_fp8: a residual and a SwiGLU-backward epilogue together");
+  if (residual)
+    B200_REQUIRE(((uintptr_t)residual & 15) == 0 && ldr % 8 == 0 && ldr >= N,
+                 "gemm_fp8: residual must be 16-byte aligned with a row stride (%lld) >= N, multiple of 8", ldr);
+  if (glu)
+    B200_REQUIRE(((uintptr_t)glu & 15) == 0 && ld_glu % 8 == 0 && ld_glu >= 2LL * N && ldc >= 2LL * N,
+                 "gemm_fp8 (swiglu_bwd epilogue): gate|up 16-byte aligned, rows of gate|up and C at least 2F wide");
+  else
+    B200_REQUIRE(ldc >= N, "gemm_fp8: ldc (%lld) < N (%d)", ldc, N);
+  GemmLaunch L;
+  const uint32_t box8[2] = {FP8_BK, GEMM_BM};
+  const uint64_t a_dims[2] = {(uint64_t)K, (uint64_t)M}, a_str[1] = {(uint64_t)lda};
+  int rc = make_tmap_u8(&L.tmA, A, 2, a_dims, a_str, box8);
+  if (rc) return rc;
+  const uint64_t b_dims[2] = {(uint64_t)K, (uint64_t)N}, b_str[1] = {(uint64_t)ldb};
+  rc = make_tmap_u8(&L.tmB, B, 2, b_dims, b_str, box8);
+  if (rc) return rc;
+  L.tmA2 = L.tmA;
+  L.tmB2 = L.tmB;
+  if (K2 > 0) {
+    B200_REQUIRE(A2 && B2, "gemm_fp8: second source missing");
+    B200_REQUIRE(lda2 % 8 == 0 && ldb2 % 8 == 0, "gemm_fp8: lda2/ldb2 must be multiples of 8");
+    B200_REQUIRE(n_sub == 0 || (n_sub % 128 == 0 && r > 0 && N % n_sub == 0),
+                 "gemm_fp8: n_sub (%d) must divide N and be a multiple of the 128-column tile", n_sub);
+    rc = operand_tmap(&L.tmA2, A2, lda2, false, M, n_sub > 0 ? (N / n_sub) * r : K2, GEMM_BM);
+    if (rc) return rc;
+    rc = operand_tmap(&L.tmB2, B2, ldb2, b_t != 0, N, K2, 128);
+    if (rc) return rc;
+  }
+  const uint32_t box[2] = {64, 64};
+  const uint64_t c_dims[2] = {(uint64_t)(glu ? 2LL * N : N), (uint64_t)M}, c_str[1] = {(uint64_t)ldc * 2};
+  rc = make_tmap_bf16(&L.tmC, C, 2, c_dims, c_str, box);
+  if (rc) return rc;
+  L.tmR = L.tmC;
+  if (glu || residual) {
+    const uint64_t r_str[1] = {(uint64_t)(glu ? ld_glu : ldr) * 2};
+    rc = make_tmap_bf16(&L.tmR, glu ? glu : residual, 2, c_dims, r_str, box);
+    if (rc) return rc;
+  }
+  L.M = M;
+  L.N = N;
+  L.K = K;
+  L.src2.K2 = K2 > 0 ? K2 : 0;
+  L.src2.r = r;
+  L.src2.n_sub = n_sub;
+  L.epi = GemmEpilogue{};
+  L.epi.alpha = 1.0f;
+  L.epi.group_m = g_group_m;
+  if (g_l2 < 0) l2_auto_policy(M, N, K, &L.epi.l2, &L.epi.group_m);
+  else L.epi.l2 = g_l2 & 0x4f;
+  L.stream = (cudaStream_t)stream;
+  Fp8Scales sc;
+  sc.sa = sa;
+  sc.ld_sa = ld_sa;
+  sc.sb = sb;
+  // block scales of W [N_w, K_w] are [N_w / 128][K_w / 128]; b_t: B is W^T, its output block indexes K_w
+  sc.sb_n = b_t ? 1 : K / 128;
+  sc.sb_k = b_t ? N / 128 : 1;
+  const int kind = glu ? EPI_GLU : residual ? EPI_RESIDUAL : EPI_PLAIN;
+  if (b_t) {
+    if (kind == EPI_GLU) return launch_fp8<EPI_GLU, true>(L, sc);
+    if (kind == EPI_RESIDUAL) return launch_fp8<EPI_RESIDUAL, true>(L, sc);
+    return launch_fp8<EPI_PLAIN, true>(L, sc);
+  }
+  if (kind == EPI_GLU) return launch_fp8<EPI_GLU, false>(L, sc);
+  if (kind == EPI_RESIDUAL) return launch_fp8<EPI_RESIDUAL, false>(L, sc);
+  return launch_fp8<EPI_PLAIN, false>(L, sc);
 }

@@ -66,8 +66,8 @@ static EncodeTiledFn resolve_encode() {
   return fn;
 }
 
-int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                   const uint64_t* strides_bytes, const uint32_t* box) {
+static int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box) {
   EncodeTiledFn fn = resolve_encode();
   if (!fn) return -3;
   cuuint64_t gdims[5];
@@ -91,7 +91,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
       return -1;
     }
   }
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base),
+  CUresult r = fn(out, dtype, (cuuint32_t)rank, const_cast<void*>(base),
                   gdims, gstr, gbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -102,6 +102,15 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
     return -3;
   }
   return 0;
+}
+
+int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                   const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box);
+}
+int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box);
 }
 
 }  // namespace b200

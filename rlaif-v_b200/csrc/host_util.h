@@ -37,5 +37,8 @@ cudaError_t configure_smem_once(const void* func, int bytes);
 // rank-1 entries (stride of dim 1, dim 2). Returns 0 on success.
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                    const uint64_t* strides_bytes, const uint32_t* box);
+// The same for one-byte elements (FP8 e4m3 codes): dims and box count bytes.
+int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_bytes, const uint32_t* box);
 
 }  // namespace b200

@@ -1377,6 +1377,111 @@ __global__ void dropout_rows_kernel(const bf16* x, const bf16* __restrict__ g, b
   }
 }
 
+// ---- FP8 e4m3 quantization of the frozen base's GEMM operands (DESIGN.md §3 "FP8 frozen base") ----
+// A tile (1 x 128 of a row, or a 128 x 128 weight block) with amax = max|x| gets the scale s = 2^e, e the smallest
+// integer with amax <= 448 * 2^e, clamped to [-126, 127] (s = 1 when amax = 0). x / s is exact and |x / s| <= 448,
+// so the code RNE_e4m3(x / s) never saturates. oracle/fp8_oracle.py is the reference of every code and scale.
+__device__ __forceinline__ int fp8_scale_exp(float amax) {
+  if (!(amax > 0.f)) return 0;
+  int E;
+  const float m = frexpf(amax, &E);          // amax = m * 2^E, m in [0.5, 1); 448 = 0.875 * 2^9
+  const int e = m <= 0.875f ? E - 9 : E - 8;
+  return e < -126 ? -126 : (e > 127 ? 127 : e);
+}
+// two codes, RNE (lo in the low byte)
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+__device__ __forceinline__ uint2 e4m3x8(const float (&v)[8], float inv) {
+  uint2 q;
+  q.x = e4m3x2(v[0] * inv, v[1] * inv) | (e4m3x2(v[2] * inv, v[3] * inv) << 16);
+  q.y = e4m3x2(v[4] * inv, v[5] * inv) | (e4m3x2(v[6] * inv, v[7] * inv) << 16);
+  return q;
+}
+
+// One half-warp per 1 x 128 tile (16 lanes x one 16-byte load of 8 bf16); tile t = kb * M + m, so the scales of one
+// K-block are written row after row. s: [K / 128][ld_s].
+__global__ void __launch_bounds__(256) quant_fp8_rows_kernel(const bf16* __restrict__ x, long long ldx,
+                                                             uint8_t* __restrict__ q, long long ldq,
+                                                             float* __restrict__ s, long long ld_s, int M, int KB) {
+  const int l = threadIdx.x & 15;
+  const long long n_tiles = (long long)M * KB;
+  // whole warps step together (the amax shuffle takes all 32 lanes); a half past the last tile idles
+  for (long long t = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 4; t - (threadIdx.x >> 4 & 1) < n_tiles;
+       t += ((long long)gridDim.x * blockDim.x) >> 4) {
+    const bool live = t < n_tiles;
+    const int kb = live ? (int)(t / M) : 0, m = live ? (int)(t - (long long)kb * M) : 0;
+    const long long col = (long long)kb * 128 + l * 8;
+    float v[8];
+    if (live) {
+      load8(x + m * ldx + col, v);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = 0.f;
+    }
+    float a = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a = fmaxf(a, fabsf(v[j]));
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+    const int e = fp8_scale_exp(a);
+    if (!live) continue;
+    *reinterpret_cast<uint2*>(q + m * ldq + col) = e4m3x8(v, ldexpf(1.f, -e));
+    if (l == 0) s[(long long)kb * ld_s + m] = ldexpf(1.f, e);
+  }
+}
+
+// One CTA per 128 x 128 block of W [N, K]: W codes, W^T codes (through shared memory) and the block's scale
+// s[nb * ld_s + kb]. Runs once per matrix when the model loads.
+__global__ void __launch_bounds__(256) quant_fp8_blocks_kernel(const bf16* __restrict__ w, long long ldw,
+                                                               uint8_t* __restrict__ q, long long ldq,
+                                                               uint8_t* __restrict__ qt, long long ldt,
+                                                               float* __restrict__ s, long long ld_s) {
+  __shared__ uint8_t tile[128][128 + 8];
+  __shared__ float red[8];
+  const int kb = blockIdx.x, nb = blockIdx.y, tid = threadIdx.x;
+  const bf16* src = w + (long long)nb * 128 * ldw + kb * 128;
+  float v[8][8];
+  float a = 0.f;
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {
+    const int idx = it * 256 + tid, row = idx >> 4, c8 = (idx & 15) * 8;
+    load8(src + row * ldw + c8, v[it]);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a = fmaxf(a, fabsf(v[it][j]));
+  }
+  a = warp_max(a);
+  if ((tid & 31) == 0) red[tid >> 5] = a;
+  __syncthreads();
+  a = red[0];
+#pragma unroll
+  for (int i = 1; i < 8; ++i) a = fmaxf(a, red[i]);
+  const int e = fp8_scale_exp(a);
+  const float inv = ldexpf(1.f, -e);
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {
+    const int idx = it * 256 + tid, row = idx >> 4, c8 = (idx & 15) * 8;
+    const uint2 c = e4m3x8(v[it], inv);
+    *reinterpret_cast<uint2*>(q + ((long long)nb * 128 + row) * ldq + kb * 128 + c8) = c;
+    *reinterpret_cast<uint2*>(&tile[row][c8]) = c;
+  }
+  if (tid == 0) s[(long long)nb * ld_s + kb] = ldexpf(1.f, e);
+  __syncthreads();
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {        // W^T row kb*128 + k: 8 consecutive n per thread
+    const int idx = it * 256 + tid, k = idx >> 4, n8 = (idx & 15) * 8;
+    uint32_t lo = 0, hi = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      lo |= (uint32_t)tile[n8 + j][k] << (8 * j);
+      hi |= (uint32_t)tile[n8 + 4 + j][k] << (8 * j);
+    }
+    *reinterpret_cast<uint2*>(qt + ((long long)kb * 128 + k) * ldt + nb * 128 + n8) = make_uint2(lo, hi);
+  }
+}
+
 static inline int grid_for(long long work_items, int threads, int max_blocks_per_sm = 8) {
   long long blocks = (work_items + threads - 1) / threads;
   long long cap = (long long)num_sms() * max_blocks_per_sm;
@@ -2043,6 +2148,40 @@ extern "C" int rlaifv_dropout_rows_bwd_add(void* dx, const void* g, const int* r
   B200_REQUIRE(width % 8 == 0 && n_rows > 0 && p >= 0.f && p < 1.f, "dropout_rows_bwd_add: width %% 8 != 0 or bad p");
   dropout_rows_kernel<<<grid_for(n_rows * (width / 8), 256), 256, 0, ST>>>(
       (const bf16*)dx, (const bf16*)g, (bf16*)dx, rows, n_rows, width / 8, dropout_threshold(p), 1.f / (1.f - p), seed);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int rlaifv_quant_fp8_rows(const void* x, long long ldx, void* q, long long ldq, float* s, long long ld_s,
+                                     int M, int K, void* stream) {
+  B200_REQUIRE(x && q && s, "quant_fp8_rows: null pointer");
+  B200_REQUIRE(M > 0 && K > 0 && K % 128 == 0, "quant_fp8_rows: K (%d) must be a positive multiple of 128", K);
+  B200_REQUIRE(ldx >= K && ldx % 8 == 0 && ((uintptr_t)x & 15) == 0,
+               "quant_fp8_rows: x must be 16-byte aligned with a row stride (%lld) >= K, multiple of 8", ldx);
+  B200_REQUIRE(ldq >= K && ldq % 16 == 0 && ((uintptr_t)q & 15) == 0,
+               "quant_fp8_rows: codes must be 16-byte aligned with a row stride (%lld) >= K, multiple of 16", ldq);
+  B200_REQUIRE(ld_s >= M && ld_s % 4 == 0 && ((uintptr_t)s & 15) == 0,
+               "quant_fp8_rows: scales need ld_s (%lld) >= M (%d), a multiple of 4, 16-byte aligned", ld_s, M);
+  const long long threads = (long long)M * (K / 128) * 16;
+  quant_fp8_rows_kernel<<<grid_for(threads, 256), 256, 0, ST>>>((const bf16*)x, ldx, (uint8_t*)q, ldq, s, ld_s, M,
+                                                                 K / 128);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int rlaifv_quant_fp8_blocks(const void* w, long long ldw, void* q, long long ldq, void* qt, long long ldt,
+                                       float* s, long long ld_s, int N, int K, void* stream) {
+  B200_REQUIRE(w && q && qt && s, "quant_fp8_blocks: null pointer");
+  B200_REQUIRE(N > 0 && K > 0 && N % 128 == 0 && K % 128 == 0,
+               "quant_fp8_blocks: N (%d) and K (%d) must be positive multiples of 128", N, K);
+  B200_REQUIRE(ldw >= K && ldw % 8 == 0 && ((uintptr_t)w & 15) == 0,
+               "quant_fp8_blocks: W must be 16-byte aligned with a row stride (%lld) >= K, multiple of 8", ldw);
+  B200_REQUIRE(ldq >= K && ldq % 8 == 0 && ((uintptr_t)q & 7) == 0 && ldt >= N && ldt % 8 == 0 &&
+                   ((uintptr_t)qt & 7) == 0,
+               "quant_fp8_blocks: code buffers must be 8-byte aligned, row strides multiples of 8 covering K / N");
+  B200_REQUIRE(ld_s >= K / 128, "quant_fp8_blocks: ld_s (%lld) < K / 128", ld_s);
+  quant_fp8_blocks_kernel<<<dim3(K / 128, N / 128), 256, 0, ST>>>((const bf16*)w, ldw, (uint8_t*)q, ldq,
+                                                                   (uint8_t*)qt, ldt, s, ld_s);
   B200_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -119,6 +119,11 @@ _SIGNATURES = {
     "rlaifv_rope_pos_bwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_void_p],
     "rlaifv_dropout_rows_fwd": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, ctypes.c_ulonglong, c_void_p],
     "rlaifv_dropout_rows_bwd_add": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, ctypes.c_ulonglong, c_void_p],
+    "rlaifv_quant_fp8_rows": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p],
+    "rlaifv_quant_fp8_blocks": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p],
+    "rlaifv_gemm_fp8": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                        c_int, c_int, c_int, c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                        c_void_p],
 }
 _INT_RETURNING_PLAIN = {"rlaifv_rmsnorm_bwd_partials": []}
 

@@ -23,9 +23,9 @@ _BF = torch.bfloat16
 
 
 class LlavaLlamaForCausalLM:
-    def __init__(self, dims: LlavaDims = None, device="cuda", hf_state=None, seed=0):
+    def __init__(self, dims: LlavaDims = None, device="cuda", hf_state=None, seed=0, base_fp8=False):
         self.dims = dims or LlavaDims()
-        self.policy = LlavaDPOPolicy(self.dims, device, hf_state=hf_state, seed=seed)
+        self.policy = LlavaDPOPolicy(self.dims, device, hf_state=hf_state, seed=seed, base_fp8=base_fp8)
         self.device = self.policy.device
         self.dtype = _BF
         self.training = True

@@ -155,27 +155,38 @@ class FlatStore:
             v.copy_(state[k].to(device=v.device, dtype=_BF))
 
 
+# the decoder's frozen-base matrices of one layer (an FP8 base keeps them in Fp8BaseStore instead)
+BASE_GROUPS = ("qkv", "o", "gu", "down")
+
+
 class ParamStore(FlatStore):
     """The decoder's (and LLaVA's projector's) parameters and gradients.
 
     Storage tensors: embed, per layer {qkv [3H,H], o [H,H], gu [2F,H], down [H,F], ln1 [H], ln2 [H]},
     norm [H], lm_head [V,H], projector {w0 [H,C], w2 [H,H], b0 [H], b2 [H]}.
     HF state-dict names map onto (views of) these — see hf_views().
+    base=False (FP8 frozen base): the layers hold only ln1 / ln2; qkv, o, gu and down live in Fp8BaseStore and have
+    neither a bf16 copy nor gradient storage.
     """
 
-    def __init__(self, dims: LlavaDims, device):
-        self.dims = d = dims
+    def __init__(self, dims: LlavaDims, device, base=True):
+        self.dims = dims
+        self.base = base
+        super().__init__(self.layout(dims, base), device)
+
+    @staticmethod
+    def layout(d, base=True):
         H, F, V, C, KV = d.hidden_size, d.intermediate_size, d.vocab_size, d.clip_hidden, d.kv_size
         layout = [("embed", [("embed", (V, H))], [])]
         layout += [(f"layer{i}",
                     [(f"l{i}.qkv", (H + 2 * KV, H)), (f"l{i}.o", (H, H)), (f"l{i}.gu", (2 * F, H)),
-                     (f"l{i}.down", (H, F))],
+                     (f"l{i}.down", (H, F))] if base else [],
                     [(f"l{i}.ln1", (H,)), (f"l{i}.ln2", (H,))]) for i in range(d.num_layers)]
         layout.append(("head", [("lm_head", (V, H))], [("norm", (H,))]))
         if d.frontend == "clip_mlp":
             layout.append(("projector", [("proj.w0", (H, C)), ("proj.w2", (H, H))],
                            [("proj.b0", (H,)), ("proj.b2", (H,))]))
-        super().__init__(layout, device)
+        return layout
 
     def hf_views(self, grads=False):
         """HF state-dict name -> view into the fused parameter (or, with grads, gradient) storage
@@ -189,6 +200,10 @@ class ParamStore(FlatStore):
                         "model.mm_projector.2.weight": src["proj.w2"], "model.mm_projector.2.bias": src["proj.b2"]})
         for i in range(d.num_layers):
             pre = f"model.layers.{i}."
+            out[pre + "input_layernorm.weight"] = src[f"l{i}.ln1"]
+            out[pre + "post_attention_layernorm.weight"] = src[f"l{i}.ln2"]
+            if not self.base:
+                continue
             qkv, gu = src[f"l{i}.qkv"], src[f"l{i}.gu"]
             out[pre + "self_attn.q_proj.weight"] = qkv[0:H]
             out[pre + "self_attn.k_proj.weight"] = qkv[H:H + KV]
@@ -197,12 +212,54 @@ class ParamStore(FlatStore):
             out[pre + "mlp.gate_proj.weight"] = gu[0:F]
             out[pre + "mlp.up_proj.weight"] = gu[F:2 * F]
             out[pre + "mlp.down_proj.weight"] = src[f"l{i}.down"]
-            out[pre + "input_layernorm.weight"] = src[f"l{i}.ln1"]
-            out[pre + "post_attention_layernorm.weight"] = src[f"l{i}.ln2"]
         return out
 
     def hf_grad_views(self):
         return self.hf_views(grads=True)
+
+
+class Fp8BaseStore:
+    """The decoder's frozen-base matrices in e4m3 (DESIGN.md §3 "FP8 frozen base"): per layer one ops.Fp8Weight each
+    for qkv [H+2KV, H], o [H, H], gu [2F, H] and down [H, F], quantized one HF tensor at a time as they arrive (the
+    128-row blocks of q / k / v and of gate / up never straddle two of them: H and F are multiples of 128)."""
+
+    # HF linear of layer i -> (group, first row of its block of the fused matrix)
+    @staticmethod
+    def hf_rows(d):
+        H, F, KV = d.hidden_size, d.intermediate_size, d.kv_size
+        return {"self_attn.q_proj": ("qkv", 0), "self_attn.k_proj": ("qkv", H), "self_attn.v_proj": ("qkv", H + KV),
+                "self_attn.o_proj": ("o", 0), "mlp.gate_proj": ("gu", 0), "mlp.up_proj": ("gu", F),
+                "mlp.down_proj": ("down", 0)}
+
+    @staticmethod
+    def check_dims(d):
+        H, F, KV = d.hidden_size, d.intermediate_size, d.kv_size
+        if H % 128 or F % 128 or KV % 128:
+            raise ValueError("base_fp8: hidden_size (%d), intermediate_size (%d) and the k/v width (%d) must be "
+                             "multiples of 128 (the FP8 block size)" % (H, F, KV))
+
+    def __init__(self, dims: LlavaDims, device):
+        self.check_dims(dims)
+        d = self.dims = dims
+        H, F, KV = d.hidden_size, d.intermediate_size, d.kv_size
+        shapes = {"qkv": (H + 2 * KV, H), "o": (H, H), "gu": (2 * F, H), "down": (H, F)}
+        self.w = [{g: ops.Fp8Weight(*shapes[g], device) for g in BASE_GROUPS} for _ in range(d.num_layers)]
+
+    def quantize(self, i, group, row0, w):
+        """Rows [row0, row0 + w.shape[0]) of layer i's `group` matrix from the bf16 (device) tensor w."""
+        ops.quant_fp8_blocks(w, *self.w[i][group].rows(row0, w.shape[0]))
+
+    def load_hf(self, state):
+        """Stream the 7 HF linears of each layer through the quantizer, one tensor on the device at a time."""
+        dev = self.w[0]["qkv"].q.device
+        for i in range(self.dims.num_layers):
+            for name, (group, row0) in self.hf_rows(self.dims).items():
+                w = state[f"model.layers.{i}.{name}.weight"].to(device=dev, dtype=_BF).contiguous()
+                self.quantize(i, group, row0, w)
+                del w
+
+    def nbytes(self):
+        return sum(w.nbytes() for layer in self.w for w in layer.values())
 
 
 class LoraStore(FlatStore):
@@ -426,13 +483,19 @@ class ClipWeights:
 class LlavaDPOPolicy:
     """Forward (policy log-probs) and backward (gradients into ParamStore.grad) of one micro-batch."""
 
-    def __init__(self, dims: LlavaDims, device="cuda", hf_state=None, seed=0, init_std=0.02):
+    def __init__(self, dims: LlavaDims, device="cuda", hf_state=None, seed=0, init_std=0.02, base_fp8=False):
         self.dims = dims
         self.device = torch.device(device)
-        self.store = ParamStore(dims, self.device)
+        # base_fp8: the decoder's qkv / o / gu / down are stored only in e4m3 (Fp8BaseStore) and their forward and dgrad
+        # GEMMs run on FP8 tensor cores; trains only with LoRA (the base gets no gradient)
+        self.base_fp8 = bool(base_fp8)
+        self.fp8 = Fp8BaseStore(dims, self.device) if self.base_fp8 else None
+        self.store = ParamStore(dims, self.device, base=not self.base_fp8)
         has_clip = dims.frontend == "clip_mlp"
         if hf_state is not None:
             self.store.load_hf(hf_state)
+            if self.fp8 is not None:
+                self.fp8.load_hf(hf_state)
             self.clip = ClipWeights(dims, self.device, hf_state) if has_clip else None
         else:
             self._random_init(seed, init_std)
@@ -487,8 +550,14 @@ class LlavaDPOPolicy:
     # ---- what the optimizer trains / in which order the forward needs it ----
     def trainable_buckets(self):
         if self.lora is None:
+            self._refuse_fp8_full()
             return self.store.opt_buckets()
         return self.lora.opt_buckets() + self.store.opt_buckets(names={"projector"})
+
+    def _refuse_fp8_full(self):
+        if self.base_fp8:
+            raise ValueError("base_fp8: an FP8 frozen base trains only with LoRA adapters (enable_lora); full "
+                             "fine-tuning needs the bf16 base weights and their gradients")
 
     def param_need_order(self):
         d = self.dims
@@ -503,6 +572,10 @@ class LlavaDPOPolicy:
         from .zero2 import activation_reserve_bytes
         d = self.dims
         reserve = activation_reserve_bytes(d, pairs, seq_len, self.stash_act)
+        if self.base_fp8:
+            # one reused pair of FP8 scratch buffers: codes (1 B) and row scales (4 B per 128) of the widest input
+            widest = max(d.hidden_size + 2 * d.kv_size, 2 * d.intermediate_size)
+            reserve += 2 * pairs * seq_len * widest * (1 + 4 / 128)
         if self.lora is None:
             reserve += 4 * d.vocab_size * d.hidden_size
         return reserve
@@ -521,9 +594,10 @@ class LlavaDPOPolicy:
     def _lin_fwd(self, i, group, x, out, residual=None, ls=None):
         """out = x @ W^T (+ residual). LoRA: t = s * x @ A^T (all sub-linears' lora_A stacked), then ONE GEMM
         accumulates x @ W^T and t_j @ B_j^T in the same accumulator tile (rlaifv_gemm_bf16_dual)."""
-        W = self.store.p[f"l{i}.{group}"]
         if self.lora is None:
-            return ops.gemm(x, W, out, residual=residual)
+            if self.base_fp8:
+                return ops.gemm_fp8(*self._fp8_quant(x), self.fp8.w[i][group], out, residual=residual)
+            return ops.gemm(x, self.store.p[f"l{i}.{group}"], out, residual=residual)
         L = self.lora
         a_name, b_names, bcat = self._GROUPS[group]
         A = L.p[f"l{i}.{a_name}"]
@@ -539,7 +613,12 @@ class LlavaDPOPolicy:
             ls["seed_" + group] = seed
         ops.gemm(xa, A, t, alpha=L.scaling)
         n_sub = out.shape[1] // len(b_names) if len(b_names) > 1 else 0
-        ops.gemm_dual(x, W, t, L.p[f"l{i}.{bcat}"], out, k2=L.r, r=L.r, n_sub=n_sub, residual=residual)
+        if self.base_fp8:
+            ops.gemm_fp8(*self._fp8_quant(x), self.fp8.w[i][group], out, a2=t, b2=L.p[f"l{i}.{bcat}"], k2=L.r, r=L.r,
+                         n_sub=n_sub, residual=residual)
+        else:
+            ops.gemm_dual(x, self.store.p[f"l{i}.{group}"], t, L.p[f"l{i}.{bcat}"], out, k2=L.r, r=L.r, n_sub=n_sub,
+                          residual=residual)
         if ls is not None:
             ls["t_" + group] = t
         return out
@@ -548,13 +627,15 @@ class LlavaDPOPolicy:
         """dx = dy @ W (+ adapter path); weight gradients: base (full FT) or adapters (LoRA).
         glu (down projection only): the layer's gate|up pre-activations [M, 2F]; dx_out is then [M, 2F] and receives
         swiglu_bwd(glu, dy @ W) from the GEMM epilogue — d(act) stays in the accumulator (ops.gemm_swiglu_bwd)."""
-        W = self.store.p[f"l{i}.{group}"]
         if self.lora is None:
+            self._refuse_fp8_full()
+            W = self.store.p[f"l{i}.{group}"]
             ops.gemm(dy, x, self.store.g[f"l{i}.{group}"], a_mn=True, b_mn=True, accumulate=acc)
             if glu is not None:
                 return ops.gemm_swiglu_bwd(dy, W, glu, dx_out)
             return ops.gemm(dy, W, dx_out, b_mn=True)
         L = self.lora
+        W = None if self.base_fp8 else self.store.p[f"l{i}.{group}"]
         a_name, b_names, _ = self._GROUPS[group]
         A = L.p[f"l{i}.{a_name}"]
         r, M = L.r, x.shape[0]
@@ -572,22 +653,44 @@ class LlavaDPOPolicy:
                                  rows=ls.get("rows"))
             ops.gemm(dt, xd, L.g[f"l{i}.{a_name}"], a_mn=True, b_mn=True, accumulate=acc)             # dA = dt^T drop(x)
             dx_plain = dx_out if glu is None else self.buf("dact", tuple(x.shape))
-            ops.gemm(dy, W, dx_plain, b_mn=True)
+            if self.base_fp8:
+                ops.gemm_fp8(*self._fp8_quant(dy), self.fp8.w[i][group], dx_plain, dgrad=True)
+            else:
+                ops.gemm(dy, W, dx_plain, b_mn=True)
             pa = ops.gemm(dt, A, self.buf("lora_xd_%d" % x.shape[1], tuple(x.shape)), b_mn=True)                       # dt @ A
             ops.dropout_bwd_add(dx_plain, pa, L.dropout, seed, rows=ls.get("rows"))
             return dx_plain if glu is None else ops.swiglu_bwd(glu, dx_plain, dx_out)
         ops.gemm(dt, x, L.g[f"l{i}.{a_name}"], a_mn=True, b_mn=True, accumulate=acc)                  # dA = dt^T x
         # dx = dy @ W + dt @ A in one pass (second source = stacked lora_A, MN-major like W)
+        if self.base_fp8:
+            return ops.gemm_fp8(*self._fp8_quant(dy), self.fp8.w[i][group], dx_out, dgrad=True, a2=dt, b2=A,
+                                k2=A.shape[0], glu=glu)
         if glu is not None:
             return ops.gemm_swiglu_bwd(dy, W, glu, dx_out, a2=dt, b2=A)
         return ops.gemm_dual(dy, W, dt, A, dx_out, k2=A.shape[0], r=r, n_sub=0, b_mn=True)
 
     # ------------------------------------------------------------------ init / buffers
+    def _fp8_quant(self, x):
+        """(codes, row scales) of a GEMM input, in one pair of buffers every frozen-base GEMM reuses (each consumes
+        them before the next quantization on the same stream)."""
+        d = self.dims
+        M, K = x.shape
+        widest = max(d.hidden_size + 2 * d.kv_size, 2 * d.intermediate_size)
+        q = self.buf("fp8_q", (M * widest,), torch.float8_e4m3fn)[:M * K].view(M, K)
+        Mp = ops.fp8_scale_rows(M)
+        s = self.buf("fp8_s", (Mp * (widest // 128),), _F32)[:Mp * (K // 128)].view(K // 128, Mp)
+        return ops.quant_fp8_rows(x, q, s)
+
     def _random_init(self, seed, std):
+        """The bf16 layout's draws in its order, so a bf16 and an FP8 policy of one seed hold the same weights (an FP8
+        base matrix is drawn into a temporary and quantized right away)."""
         g = torch.Generator(device=self.device).manual_seed(seed)
-        for b in self.store.buckets:
-            for s in b.segments:
-                v = self.store.p[s.name]
+        for _, decay, nodecay in ParamStore.layout(self.dims):
+            for name, shape in decay + nodecay:
+                s = Segment(name, shape, 0, True)
+                v = self.store.p.get(name)
+                if v is None:
+                    v = torch.empty(shape, dtype=_BF, device=self.device)
                 if len(s.shape) == 1 and (s.name.endswith("ln1") or s.name.endswith("ln2") or s.name == "norm"):
                     v.fill_(1.0)
                 elif len(s.shape) == 1:
@@ -599,6 +702,9 @@ class LlavaDPOPolicy:
                     for o in range(0, flat.numel(), step):
                         n = min(step, flat.numel() - o)
                         flat[o:o + n].copy_(torch.randn(n, generator=g, device=self.device, dtype=_F32) * std)
+                    if name not in self.store.p:
+                        i, group = name[1:].split(".")
+                        self.fp8.quantize(int(i), group, 0, v)
 
     def buf(self, key, shape, dtype=_BF):
         t = self._bufs.get(key)

@@ -666,3 +666,88 @@ def dropout_bwd_add(dx, g, p, seed, rows=None):
         return dx
     _l.call("rlaifv_dropout_bwd_add", _l.ptr(dx), _l.ptr(g), dx.numel(), float(p), int(seed), _l.stream_ptr())
     return dx
+
+
+# --------------------------------------------------------------------------------------------
+# FP8 (e4m3) frozen base (DESIGN.md §3 "FP8 frozen base"; the format: include/rlaifv_b200.h)
+# --------------------------------------------------------------------------------------------
+_E4M3 = torch.float8_e4m3fn
+
+
+class Fp8Weight:
+    """A frozen weight W [N, K] in e4m3: codes q [N, K], the transposed codes qt [K, N] the dgrad reads, and the
+    block scales s [N/128, K/128] fp32 shared by both."""
+
+    def __init__(self, N, K, device):
+        assert N % 128 == 0 and K % 128 == 0, (N, K)
+        self.N, self.K = N, K
+        self.q = torch.empty((N, K), dtype=_E4M3, device=device)
+        self.qt = torch.empty((K, N), dtype=_E4M3, device=device)
+        self.s = torch.empty((N // 128, K // 128), dtype=_f32, device=device)
+
+    def rows(self, n0, n):
+        """(q, qt, s) views of W's rows [n0, n0 + n) (n0, n: multiples of 128), for quantizing one sub-matrix."""
+        assert n0 % 128 == 0 and n % 128 == 0
+        return self.q[n0:n0 + n], self.qt[:, n0:n0 + n], self.s[n0 // 128:(n0 + n) // 128]
+
+    def nbytes(self):
+        return self.q.numel() + self.qt.numel() + 4 * self.s.numel()
+
+
+def fp8_scale_rows(M):
+    """Row-scale leading dimension of an M-row operand: M rounded up to a multiple of 4."""
+    return (M + 3) // 4 * 4
+
+
+def quant_fp8_rows(x, q=None, s=None):
+    """x [M, K] bf16 (row stride allowed) -> (codes [M, K] e4m3, row scales [K/128, fp8_scale_rows(M)] fp32)."""
+    _chk(x)
+    M, K = x.shape
+    assert x.stride(1) == 1
+    if q is None:
+        q = torch.empty((M, K), dtype=_E4M3, device=x.device)
+    if s is None:
+        s = torch.empty((K // 128, fp8_scale_rows(M)), dtype=_f32, device=x.device)
+    _chk(q, _E4M3), _chk(s, _f32)
+    assert q.shape == (M, K) and q.stride(1) == 1 and s.shape[0] == K // 128 and s.shape[1] >= M and s.stride(1) == 1
+    _l.call("rlaifv_quant_fp8_rows", _l.ptr(x), x.stride(0), _l.ptr(q), q.stride(0), _l.ptr(s), s.stride(0), M, K,
+            _l.stream_ptr())
+    return q, s
+
+
+def quant_fp8_blocks(w, q, qt, s):
+    """W [N, K] bf16 -> codes q [N, K], transposed codes qt [K, N] and block scales s [N/128, K/128] (views of a wider
+    Fp8Weight allowed: Fp8Weight.rows)."""
+    _chk(w), _chk(q, _E4M3), _chk(qt, _E4M3), _chk(s, _f32)
+    N, K = w.shape
+    assert w.stride(1) == 1 and q.shape == (N, K) and qt.shape == (K, N) and s.shape == (N // 128, K // 128)
+    assert q.stride(1) == 1 and qt.stride(1) == 1 and s.stride(1) == 1
+    _l.call("rlaifv_quant_fp8_blocks", _l.ptr(w), w.stride(0), _l.ptr(q), q.stride(0), _l.ptr(qt), qt.stride(0),
+            _l.ptr(s), s.stride(0), N, K, _l.stream_ptr())
+
+
+def gemm_fp8(aq, sa, w, out, *, dgrad=False, a2=None, b2=None, k2=0, r=0, n_sub=0, residual=None, glu=None):
+    """out [M, N] = dequant(aq, sa) @ op(W)^T (+ a2[:, koff:koff+k2] @ op(b2)^T) (+ residual), W an Fp8Weight.
+    Forward (dgrad=False): op(W) = W, N = W.N, b2 [N, r] K-major. dgrad: op(W) = W^T (read from w.qt), N = W.K,
+    b2 [k2, N] MN-major. glu ([gate | up] [M, 2N]): out [M, 2N] receives the SwiGLU backward of the product."""
+    _chk(aq, _E4M3), _chk(sa, _f32), _chk(out)
+    M, K = aq.shape
+    B = w.qt if dgrad else w.q
+    N = B.shape[0]
+    assert B.shape[1] == K and aq.stride(1) == 1 and out.stride(1) == 1 and sa.shape[0] == K // 128
+    assert out.shape == ((M, 2 * N) if glu is not None else (M, N))
+    if a2 is not None:
+        _chk(a2), _chk(b2)
+        assert k2 > 0
+    if residual is not None:
+        _chk(residual)
+        assert residual.shape == (M, N) and residual.stride(1) == 1
+    if glu is not None:
+        _chk(glu)
+        assert glu.shape == (M, 2 * N) and glu.stride(1) == 1
+    _l.call("rlaifv_gemm_fp8", _l.ptr(aq), aq.stride(0), _l.ptr(sa), sa.stride(0), _l.ptr(B), B.stride(0), _l.ptr(w.s),
+            int(dgrad), _l.ptr(a2), a2.stride(0) if a2 is not None else 0, _l.ptr(b2),
+            b2.stride(0) if b2 is not None else 0, int(k2) if a2 is not None else 0, int(r), int(n_sub), _l.ptr(out),
+            out.stride(0), M, N, K, _l.ptr(residual), residual.stride(0) if residual is not None else 0, _l.ptr(glu),
+            glu.stride(0) if glu is not None else 0, _l.stream_ptr())
+    return out

@@ -114,6 +114,8 @@ class TrainingArguments:                   # muffin/train/train_llava15.py:72-10
     lora_dropout: float = 0.05
     lora_weight_path: Optional[str] = None
     lora_bias: str = "none"
+    # the decoder's frozen base matrices in FP8 e4m3 (DESIGN.md §3 "FP8 frozen base"); needs --lora_enable True
+    base_fp8: bool = False
 
 
 def _add_fields(parser, cls):
@@ -216,6 +218,11 @@ def dims_from_checkpoint(model_dir, vision_tower_dir, select_layer, max_len):
     return LlavaDims(**kw)
 
 
+def check_base_fp8(training_args):
+    if training_args.base_fp8 and not training_args.lora_enable:
+        raise ValueError("--base_fp8 True needs --lora_enable True: the FP8 base is frozen and gets no gradient")
+
+
 def init_model(model_args, data_args, training_args, attn_implementation=None, source_rows=None):
     """muffin/train/train_llava15.py:198-281: policy model (+ frozen reference used once for the
     log-prob pre-pass inside the dataset), tokenizer, data module."""
@@ -227,8 +234,11 @@ def init_model(model_args, data_args, training_args, attn_implementation=None, s
     dims = dims_from_checkpoint(model_args.model_name_or_path, model_args.vision_tower,
                                 select_layer=model_args.mm_vision_select_layer,
                                 max_len=training_args.model_max_length)
+    check_base_fp8(training_args)
     state = load_hf_checkpoint(model_args.model_name_or_path, model_args.vision_tower)
-    model = LlavaLlamaForCausalLM(dims, torch.device("cuda", local_rank), hf_state=state)
+    # the base's storage format is fixed when the model is built, before enable_lora
+    model = LlavaLlamaForCausalLM(dims, torch.device("cuda", local_rank), hf_state=state,
+                                  base_fp8=bool(training_args.base_fp8))
     model.config.use_cache = False
     model.policy.share_prefix = bool(training_args.share_prompt_prefix)
     if training_args.lora_enable:
